@@ -109,9 +109,61 @@ struct Bfly {
             Bfly<B, INV, S + 1, 0>::run(x);
     }
 };
+#ifndef MS_DFT_REPAIR_EACH
+// The same network on the redundant 96-bit form (field.cuh::L96): no repair between butterflies, one reduction per
+// output.  The Montgomery word of a twiddle is +-2^m, and a Montgomery product by it multiplies the value by
+// +-2^(m - 64) = +-2^K (2^96 = -1): K = m - 64 for m >= 64, and K = m + 32 with the sign flipped for m < 64.
+//
+// Bound, with b_s the bound on |value| entering level s (inputs are u64, so b_1 = 2^64, non-negative):
+//   level 1:   sums and differences of two inputs: |.| < 2^65
+//   level s>1: a twiddled operand W has |W| < 2^65 + b_s / 2 (l96_mul_pow2), so |u +- W| < b_s + 2^65 + b_s / 2:
+//              b_3 < 2^67, b_4 < 2^68, outputs of level 4 in (-2^69, 2^69).
+// Register 0 also carries kBias = 2^7 p (= 0 mod p, < 2^71).  In this network register 0's contents only ever reach the
+// untwiddled side of a butterfly, so every output carries exactly + kBias: outputs lie in (2^70, 2^72), non-negative and
+// below 2^95, as l96_reduce needs.
+constexpr u64 kBiasLo = P << 7;                 // 2^7 p = 2^71 - 2^39 + 2^7 as 96 bits
+constexpr u32 kBiasHi = (u32)(P >> 57);
+static_assert(kBiasHi == 127 && kBiasLo == 0xFFFFFF8000000080ULL, "2^7 p");
+template <int B, bool INV, int S, int A>
+struct BflyL {
+    static __host__ __device__ __forceinline__ void run(L96 (&x)[1 << B]) {
+        constexpr int span = 1 << (B - S);
+        if constexpr ((A & span) == 0) {
+            constexpr int j = brev_c(A >> (B - S + 1), S - 1);
+            const L96 u = x[A], v = x[A + span];
+            if constexpr (j == 0) {
+                x[A] = l96_add(u, v);
+                x[A + span] = l96_sub(u, v);
+            } else {
+                constexpr W16Shift sh = w16_shift<INV>(j * (16 >> S));
+                constexpr int K = sh.m >= 64 ? sh.m - 64 : sh.m + 32;
+                constexpr bool neg = sh.neg != (sh.m < 64);
+                const L96 t = l96_mul_pow2<K>(v);
+                x[A] = neg ? l96_sub(u, t) : l96_add(u, t);
+                x[A + span] = neg ? l96_add(u, t) : l96_sub(u, t);
+            }
+        }
+        if constexpr (A + 1 < (1 << B))
+            BflyL<B, INV, S, A + 1>::run(x);
+        else if constexpr (S < B)
+            BflyL<B, INV, S + 1, 0>::run(x);
+    }
+};
+#endif
+
+// x[k]: any u64 in; output index kappa in register brev<B>(kappa), any u64 (a Montgomery product with a canonical
+// factor, or canon, makes it canonical)
 template <int B, bool INV>
-__device__ __forceinline__ void dft_regs(u64 (&x)[1 << B]) {
+__host__ __device__ __forceinline__ void dft_regs(u64 (&x)[1 << B]) {
+#ifdef MS_DFT_REPAIR_EACH
     Bfly<B, INV, 1, 0>::run(x);
+#else
+    L96 y[1 << B];
+    for (int i = 0; i < (1 << B); i++) y[i] = l96(x[i]);
+    y[0] = l96_add(y[0], L96{(u32)kBiasLo, (u32)(kBiasLo >> 32), kBiasHi});
+    BflyL<B, INV, 1, 0>::run(y);
+    for (int i = 0; i < (1 << B); i++) x[i] = l96_reduce(y[i]);
+#endif
 }
 
 }  // namespace msntt

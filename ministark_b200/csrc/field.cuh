@@ -161,6 +161,70 @@ inline u64 sub_ll(u64 a, u64 b) {
 }
 #endif
 
+// ---- redundant 96-bit form (the in-register DFT networks of dft.cuh) ----------------------
+// A value is the signed 96-bit integer w0 + w1 * 2^32 + (s32)w2 * 2^64, congruent to the field element mod p.  Sums and
+// differences are exact 3-limb carry chains with no repair; the networks keep |value| < 2^95 (bounds in dft.cuh) and
+// reduce once per output.
+struct L96 {
+    u32 w0, w1, w2;
+};
+GL_HD L96 l96(u64 x) { return L96{(u32)x, (u32)(x >> 32), 0u}; }
+#if defined(__CUDA_ARCH__)
+__device__ __forceinline__ L96 l96_add(L96 a, L96 b) {
+    L96 r;
+    asm("add.cc.u32 %0, %3, %6;\n\taddc.cc.u32 %1, %4, %7;\n\taddc.u32 %2, %5, %8;"
+        : "=r"(r.w0), "=r"(r.w1), "=r"(r.w2) : "r"(a.w0), "r"(a.w1), "r"(a.w2), "r"(b.w0), "r"(b.w1), "r"(b.w2));
+    return r;
+}
+__device__ __forceinline__ L96 l96_sub(L96 a, L96 b) {
+    L96 r;
+    asm("sub.cc.u32 %0, %3, %6;\n\tsubc.cc.u32 %1, %4, %7;\n\tsubc.u32 %2, %5, %8;"
+        : "=r"(r.w0), "=r"(r.w1), "=r"(r.w2) : "r"(a.w0), "r"(a.w1), "r"(a.w2), "r"(b.w0), "r"(b.w1), "r"(b.w2));
+    return r;
+}
+#else
+inline L96 l96_add(L96 a, L96 b) {
+    const u64 s0 = (u64)a.w0 + b.w0, s1 = (u64)a.w1 + b.w1 + (s0 >> 32);
+    return L96{(u32)s0, (u32)s1, a.w2 + b.w2 + (u32)(s1 >> 32)};
+}
+inline L96 l96_sub(L96 a, L96 b) {
+    const u64 d0 = (u64)a.w0 - b.w0, d1 = (u64)a.w1 - b.w1 - (d0 >> 63);
+    return L96{(u32)d0, (u32)d1, a.w2 - b.w2 - (u32)(d1 >> 63)};
+}
+#endif
+// v * 2^K (mod p), K in [0, 96).  v * 2^r (r = K % 32) is the four limbs y0..y3 (y3 signed); placed q = K / 32 limbs up
+// they form Lo + Hi * 2^96 with Lo in [0, 2^96), and 2^96 = -1 gives Lo - Hi.  Lo's top limb t is folded with
+// 2^64 = 2^32 - 1, so Lo becomes (lo0 + lo1 2^32) + t 2^32 - t, in (-2^32, 2^65).  For |v| < 2^b: |Hi| <= 2^(b + K - 96)
+// <= 2^(b - 1), so the result W has |W| < 2^65 + 2^(b - 1).
+template <int K>
+GL_HD L96 l96_mul_pow2(L96 v) {
+    static_assert(K > 0 && K < 96, "shift out of range");
+    constexpr int q = K / 32, r = K % 32;
+    u32 y0, y1, y2, y3;
+    if constexpr (r == 0) {
+        y0 = v.w0, y1 = v.w1, y2 = v.w2, y3 = (u32)((int)v.w2 >> 31);
+    } else {
+        y0 = v.w0 << r;
+        y1 = (v.w1 << r) | (v.w0 >> (32 - r));
+        y2 = (v.w2 << r) | (v.w1 >> (32 - r));
+        y3 = (u32)((int)v.w2 >> (32 - r));
+    }
+    if constexpr (q == 0) {           // Lo = (y0, y1, t = y2), Hi = y3
+        const u32 s = (u32)((int)y3 >> 31);
+        return l96_sub(l96_sub(l96_add(L96{y0, y1, 0u}, L96{0u, y2, 0u}), L96{y2, 0u, 0u}), L96{y3, s, s});
+    } else if constexpr (q == 1) {    // Lo = (0, y0, t = y1), Hi = y2 + y3 2^32
+        const u32 s = (u32)((int)y3 >> 31);
+        return l96_sub(l96_sub(L96{0u, y0, 0u}, L96{y1, 0u, 0u}), l96_sub(L96{y2, y3, s}, L96{0u, y1, 0u}));
+    } else {                          // Lo = (0, 0, t = y0), Hi = y1 + y2 2^32 + y3 2^64
+        return l96_sub(l96_sub(L96{0u, y0, 0u}, L96{y0, 0u, 0u}), L96{y1, y2, y3});
+    }
+}
+// any u64 congruent to v, for 0 <= v < 2^72: v = lo + c 2^64 = lo + c (2^32 - 1), and c (2^32 - 1) < 2^40 < p is
+// canonical, so one lazy addition finishes it
+GL_HD u64 l96_reduce(L96 v) {
+    return add_lc(((u64)v.w1 << 32) | v.w0, (u64)v.w2 * 0xFFFFFFFFull);
+}
+
 // ---- Montgomery multiplication ---------------------------------------------------------
 // returns a*b*2^-64 mod p, canonical, provided a*b < p * 2^64 (i.e. one operand < p).
 GL_HD u64 mont_reduce(u64 hi, u64 lo) {
