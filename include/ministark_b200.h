@@ -72,7 +72,8 @@ const char *ms_version(void);
 /* tuning / A-B switches of the kernels (process-wide; no reference counterpart): "ntt_tma" 0|1 selects the persistent
  * TMA pipeline for the 256 x 16 tile NTT passes (default 1), "ntt_tma_groups" 2|3 consumer groups per CTA,
  * "ntt_tma_stages" 3..8 cap on its shared-memory ring; "drop_plans" (any value) frees this context's cached NTT plans and
- * their twiddle / scale tables (hundreds of MiB for 2^24-point LDE plans; rebuilt on demand). */
+ * their twiddle / scale tables (hundreds of MiB for 2^24-point LDE plans; rebuilt on demand); "drop_scratch" (any value)
+ * frees its scratch arenas (e.g. the temporary of a large single-column transform; regrown on demand). */
 int ms_set_option(ms_ctx *ctx, const char *name, int64_t value);
 /* number of kernels this context has launched so far (bench.py "gpu_launches") */
 uint64_t ms_launch_count(ms_ctx *ctx);

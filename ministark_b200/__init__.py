@@ -206,6 +206,23 @@ class Context:
                                                        root.ctypes.data))
         return root.tobytes()
 
+    def merkle_commit_block(self, cols, field, log_block_rows, log_blocks, block, ncols, nodes, block_root, col_stride=None):
+        """hash one coset block (2^log_block_rows rows at `cols`) and write its subtree into `nodes`, the heap of the
+        whole 2^(log_block_rows + log_blocks)-leaf tree; the subtree root goes to `block_root` (32 bytes)"""
+        col_stride = (1 << log_block_rows) if col_stride is None else col_stride
+        self._ck(self.lib.ms_merkle_commit_block_sha256(self.h, field, _ptr(cols), col_stride, ncols, log_block_rows,
+                                                        log_blocks, block, _ptr(nodes), _ptr(block_root)))
+
+    def lde_rows(self, coeffs, field, log_n, log_blowup, ncols, positions, offset=GENERATOR, col_stride=None, out=None):
+        """rows `positions` of the bit-reversed coset LDE of `coeffs`, evaluated from the coefficients; returns
+        (len(positions), ncols * field) words laid out like gather_rows (or fills `out`, e.g. a device tensor)"""
+        ids = np.ascontiguousarray(positions, dtype=np.uint64)
+        if out is None:
+            out = np.empty((ids.size, ncols * field), dtype=np.uint64)
+        self._ck(self.lib.ms_lde_rows(self.h, field, _ptr(coeffs), (1 << log_n) if col_stride is None else col_stride, ncols,
+                                      log_n, log_blowup, offset, ids.ctypes.data, ids.size, _ptr(out)))
+        return out
+
     def pow_grind(self, seed, bits):
         """smallest nonce >= 1 with leading_zeros(SHA-256(seed || nonce_be8)) >= bits (src/random.rs:48-55)"""
         sd = (C.c_uint8 * 32).from_buffer_copy(bytes(seed))

@@ -10,6 +10,7 @@ import re
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MS_LIB_PATH") or os.path.join(_HERE, "libministark_b200.so")   # MS_LIB_PATH: A/B builds
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h")
+STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -64,10 +65,23 @@ _SIGS = {
     "ms_fill_random": (ci, [vp, vp, sz, u64]),
 }
 
+# include/ministark_stream.h: the entry points of the streamed prover residency
+_STREAM_SIGS = {
+    "ms_merkle_commit_block_sha256": (ci, [vp, ci, vp, sz, ui, ui, ui, sz, vp, vp]),
+    "ms_lde_rows": (ci, [vp, ci, vp, sz, ui, ui, ui, u64, vp, ui, vp]),
+}
 
-def header_symbols():
-    """every function name declared in include/ministark_b200.h"""
-    text = open(HEADER_PATH).read()
+
+def bind(lib, sigs):
+    for name, (res, args) in sigs.items():
+        fn = getattr(lib, name)
+        fn.restype = res
+        fn.argtypes = args
+
+
+def header_symbols(path=HEADER_PATH):
+    """every function name declared in include/ministark_b200.h (or in the header at `path`)"""
+    text = open(path).read()
     text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
     return sorted(set(re.findall(r"\b(ms_[a-z0-9_]+)\s*\(", text)))
 
@@ -83,10 +97,8 @@ def load():
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU fallback)")
         lib = C.CDLL(LIB_PATH)
-        for name, (res, args) in _SIGS.items():
-            fn = getattr(lib, name)
-            fn.restype = res
-            fn.argtypes = args
+        bind(lib, _SIGS)
+        bind(lib, _STREAM_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -228,6 +228,17 @@ int ms_set_option(ms_ctx *c, const char *name, int64_t value) {
         ms::ntt_drop_plans(c);
         return MS_OK;
     }
+    if (!strcmp(name, "drop_scratch")) {   // free the context's scratch arenas (regrown on demand)
+        if (!c) return MS_ERR_INVALID;
+        cudaSetDevice(c->device);
+        MS_CUDA(c, cudaStreamSynchronize(c->stream));
+        for (ms::Scratch &s : c->scratch) {
+            if (s.ptr) MS_CUDA(c, cudaFree(s.ptr));
+            s.ptr = nullptr;
+            s.cap = 0;
+        }
+        return MS_OK;
+    }
     return fail(c, MS_ERR_INVALID, "unknown option %s", name);
 }
 

@@ -14,6 +14,7 @@
 #include <mutex>
 #include <cstring>
 #include "ctx.cuh"
+#include "../../include/ministark_stream.h"
 #include <algorithm>
 #include <cstring>
 #include <deque>
@@ -378,6 +379,49 @@ int ms_merkle_commit_sha256(ms_ctx *c, int field, const void *cols, size_t col_s
     return nout.finish();
 }
 
+
+// One coset block of a tree that is committed block by block (the streaming prover never holds the whole LDE): the
+// 2^log_block_rows rows are hashed into scratch, and every subtree level is written straight into its run of the global
+// heap.  Level d >= log_blocks of a tree with N = 2^(log_block_rows + log_blocks) leaves holds 2^d nodes at [2^d, 2^(d+1));
+// block b owns the cnt = 2^(d - log_blocks) consecutive ones from 2^d + b * cnt, whose children are the block's run one
+// level down.  So the leaf pairs go to [N/2 + b * nb/2, ...) and the subtree root lands at nodes[2^log_blocks + b].
+int ms_merkle_commit_block_sha256(ms_ctx *c, int field, const void *cols, size_t col_stride_elems, unsigned ncols,
+                                  unsigned log_block_rows, unsigned log_blocks, size_t block, void *nodes, void *block_root) {
+    if (!c || !cols || !nodes || !block_root) return MS_ERR_INVALID;
+    if (field != MS_FIELD_FP && field != MS_FIELD_FQ3) return fail(c, MS_ERR_INVALID, "unknown field id %d", field);
+    if (ncols == 0) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256: no columns");
+    if (log_block_rows + log_blocks > 40) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256: tree too large");
+    if (block >> log_blocks) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256: block %zu of %zu", block, (size_t)1 << log_blocks);
+    const size_t nb = (size_t)1 << log_block_rows, beta = (size_t)1 << log_blocks, N = nb << log_blocks;
+    if (ncols > 1 && col_stride_elems < nb) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256: stride < block rows");
+    Staged in(c, cols, ((size_t)(ncols - 1) * col_stride_elems + nb) * field * 8, true, false);
+    if (in.rc) return in.rc;
+    // a host heap is staged whole, both ways: the block writes only its own runs and the rest must survive
+    Staged nd(c, nodes, log_block_rows ? N * 32 : 0, true, true);
+    if (nd.rc) return nd.rc;
+    void *lv;
+    int rc = scratch_get(c, 2, nb * 32, &lv);
+    if (rc) return rc;
+    if ((rc = hash_rows_dev(c, field, in.as<u64>(), col_stride_elems, ncols, nb, (u32 *)lv))) return rc;
+    const u32 *root = (const u32 *)lv;
+    if (log_block_rows) {
+        if ((rc = upload_pad_schedule(c))) return rc;
+        const unsigned threads = 128;
+        const u32 *src = (const u32 *)lv;
+        for (size_t cnt = nb / 2; cnt >= 1; cnt >>= 1) {
+            u32 *dst = nd.as<u32>() + (cnt * beta + block * cnt) * 8;
+            MS_SHA_DISPATCH(merkle_level_kernel, (unsigned)((cnt + threads - 1) / threads), src, dst, cnt);
+            c->launches++;
+            MS_CHECK_LAUNCH(c);
+            src = dst;
+        }
+        root = src;   // nodes[beta + block]
+    }
+    MS_CUDA(c, cudaMemcpyAsync(block_root, root, 32, cudaMemcpyDefault, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    if ((rc = in.finish())) return rc;
+    return nd.finish();
+}
 
 // Commitment of a ROW-MAJOR matrix (nrows rows of row_words contiguous words): FRI layers commit rows of
 // `ff` consecutive evaluations (src/fri.rs:199-216 builds Matrix::from_arrays(chunks) only to hash those

@@ -20,6 +20,7 @@ torch is used for device buffers and the stream only.  There is no CPU fallback:
 Context constructor raises.
 """
 import copy
+import hashlib
 import time
 
 import numpy as np
@@ -30,6 +31,7 @@ from . import deep
 from . import expr as E
 from .air import Air
 from .channel import ProverChannel, PublicCoin, serialize_element
+from .cosets import block_program, coset_offsets, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
 
 P = E.P
@@ -115,9 +117,50 @@ class Stark:
         return GpuProver.shared(device).prove(self, options, witness)
 
 
+# Device memory torch does not see, kept free on top of either estimate: the NTT plans with their twiddle and scale
+# tables (hundreds of MiB for 2^24-point LDEs), the NTT temporary (at most 1.125 GiB) and the context's scratch arenas.
+MEMORY_RESERVE = 3 << 30
+
+
+def peak_bytes(n, beta, nbase, next_, fq, ce_blowup, ff=2):
+    """Peak device bytes of one proof in each residency, from the shapes: {"resident": .., "streamed": ..}.
+
+    resident: every matrix's coefficients and bit-reversed LDE, and the leaf and node arrays of every tree, live until
+    the queries, and so does the ce-domain composition column.  streamed: the coefficients, one coset block of every
+    matrix and the node arrays (no leaves; one block's leaf digests in context scratch).  Both hold the DEEP codeword and the FRI
+    layers (folded codewords and trees, a geometric series in the folding factor ff), and 16 MiB for the small buffers
+    (block roots, remainder, query rows) and the allocator's rounding."""
+    N, M = n * beta, n * ce_blowup
+    words = nbase + fq * (next_ + ce_blowup)                 # words per row over all matrices
+    ntrees = 3 if next_ else 2
+    fri = (8 * fq + 64) * N // (ff - 1)
+    common = 8 * words * n + 8 * N * fq + fri + (16 << 20)
+    return {"resident": common + 8 * M * fq + 8 * words * N + 64 * ntrees * N,
+            "streamed": common + 8 * words * n + 32 * ntrees * N + 32 * n}
+
+
+def _gib(b):
+    return f"{b / 2**30:.2f} GiB"
+
+
+class _Run:
+    """per-proof state shared by the phases of both residencies"""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
 class GpuProver:
-    """owns the device context (one in-order stream) and runs default_prove"""
+    """owns the device context (one in-order stream) and runs default_prove.
+
+    Two residencies, chosen per proof from the estimates of `peak_bytes` against `memory_available()`:
+      resident   every LDE matrix and both arrays of every Merkle tree stay in HBM until the queries (the fastest);
+      streamed   only coefficients and tree nodes stay; each coset block of the LDE is recomputed where it is needed
+                 (commitment, constraint evaluation, DEEP) and query rows come from the coefficients (ms_lde_rows).
+    Both emit the same proof bytes.  The resident path runs whenever it fits."""
     _shared = {}
+    memory_budget = None        # bytes one proof may use on the device; None: whatever the device has free
+    last_residency = None       # "resident" or "streamed": what the last proof ran
 
     @classmethod
     def shared(cls, device=0):
@@ -125,12 +168,13 @@ class GpuProver:
             cls._shared[device] = cls(device)
         return cls._shared[device]
 
-    def __init__(self, device=0):
+    def __init__(self, device=0, memory_budget=None):
         self.device = torch.device("cuda", device)
         self.stream = torch.cuda.Stream(device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self.ctx = Context(device, stream=self.stream.cuda_stream)
         self._airs = {}
+        self.memory_budget = memory_budget
 
     # ---- helpers
     def _to_device(self, a):
@@ -160,6 +204,28 @@ class GpuProver:
     def _view(self, tree, positions):
         nodes, init, sib, height = self.ctx.merkle_prove(tree.leaves, tree.nodes, tree.n, positions)
         return MerkleView(nodes, init, sib, height)
+
+    # ---- residency
+    def memory_available(self):
+        """bytes a proof may allocate: free device memory as CUDA reports it, plus what torch's allocator holds unused,
+        minus MEMORY_RESERVE, capped by memory_budget.  Off a CUDA device only memory_budget limits (None: no limit)."""
+        cap = self.memory_budget
+        if self.device.type != "cuda":
+            return float("inf") if cap is None else cap
+        free, _ = torch.cuda.mem_get_info(self.device)
+        idle = torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+        avail = free + idle - MEMORY_RESERVE
+        return avail if cap is None else min(cap, avail)
+
+    def choose_residency(self, est):
+        """"resident" if its estimate fits, else "streamed" if that fits, else ProvingError (nothing is allocated yet)"""
+        budget = self.memory_available()
+        if est["resident"] <= budget:
+            return "resident"
+        if est["streamed"] <= budget:
+            return "streamed"
+        raise ProvingError(f"the proof does not fit on the device: it needs about {_gib(est['resident'])} resident or "
+                           f"{_gib(est['streamed'])} streamed, and {_gib(budget)} is available")
 
     # ---- default_prove
     def prove(self, stark, options, witness):
@@ -201,14 +267,23 @@ class GpuProver:
             self._airs[key].num_challenges(), self._airs[key].num_composition_constraint_coeffs(), self._airs[key].trace_arguments()
         air = copy.copy(self._airs[key])
         air.public_inputs = stark.get_public_inputs()
-        channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
         fq = FP if cfg.FQ_IS_FP else FQ3
         log_n = air.log_n
         beta = options.lde_blowup_factor
         log_b = beta.bit_length() - 1
-        log_N, N = log_n + log_b, n * beta
         nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
+        residency = self.choose_residency(peak_bytes(n, beta, nbase, next_, fq, air.ce_blowup_factor, options.fri_folding_factor))
+        self.last_residency = residency
+        channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
+        r = _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
+                 beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
+                 timings=timings, t_all=t_all, cached_air=self._airs[key])
         lap("init_air")
+        return self._prove_resident(r) if residency == "resident" else self._prove_streamed(r)
+
+    def _prove_resident(self, r):
+        ctx, stark, trace, air, channel, lap = r.ctx, r.stark, r.trace, r.air, r.channel, r.lap
+        fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
 
         # ---- base trace commitment (prover.rs:46-55).  A host trace is uploaded in column chunks on a second stream
         # while the previous chunk is interpolated and extended (columns are independent until the row hash); a
@@ -246,15 +321,8 @@ class GpuProver:
         hints = air.gen_hints(challenges)
 
         # ---- extension trace commitment (prover.rs:56-72)
-        if hasattr(trace, "build_extension_columns_device"):
-            # running products / evaluations as device scans over the resident base trace (SURVEY.md §8f rank 3)
-            ext = trace.build_extension_columns_device(challenges, ctx, base)
-        else:
-            ext = trace.build_extension_columns(challenges)
+        ext = self._extension_columns(r, challenges, base)
         del base
-        num_ext = 0 if ext is None else int(ext.shape[0])
-        if num_ext != next_:
-            raise ProvingError(f"expected {next_} extension columns, got {num_ext}")
         ext_polys = ext_lde = ext_tree = None
         if ext is not None:
             ext_polys, ext_lde, ext_tree, ext_root = self._commit_columns(self._to_device(ext), fq, log_n, log_b, next_, True)
@@ -276,21 +344,194 @@ class GpuProver:
 
         # ---- composition trace (prover.rs:110-125): coefficients over the ce coset, column i = coefficients = i mod ce_blowup
         ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
-        if ce_blowup == 1:
-            comp_polys = comp_evals.view(1, n * fq)
-        else:
-            comp_polys = self._empty(ce_blowup, n * fq)
-            ctx.matrix_from_rows(comp_evals, comp_polys, fq, n, ce_blowup)
+        comp_polys = self._composition_columns(r, comp_evals)
         _, comp_lde, comp_tree, comp_root = self._commit_columns(comp_polys, fq, log_n, log_b, ce_blowup, False)
         channel.commit_composition_trace(comp_root)
         lap("composition_trace_commitment")
 
-        # ---- out-of-domain evaluations (composer.rs:43-86)
+        # ---- DEEP composition polynomial, evaluated straight over the LDE domain (composer.rs:89-188 in evaluation form)
+        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
+        ncols_all = nbase + next_ + ce_blowup
+        sz = N * 8
+        cols = [base_lde.data_ptr() + c * sz for c in range(nbase)]
+        cols += [ext_lde.data_ptr() + c * sz * fq for c in range(next_)]
+        cols += [comp_lde.data_ptr() + c * sz * fq for c in range(ce_blowup)]
+        deep_lde = self._empty(N * fq)
+        ctx.eval_constraints_ptrs(dprog, deep_lde, r.log_N, cols, [False] * nbase + [True] * (ncols_all - nbase), fq_field=fq,
+                                  offset=GEN_MONT, trace_bitrev=True, out_bitrev=True)
+        lap("deep_composition")
+
+        layers = self._fri(r, deep_lde)
+
+        # ---- queries (fri.rs:151-177, trace.rs:115-157)
+        positions = channel.get_fri_query_positions()
+        fri_proof = self._fri_queries(r, layers, positions)
+        queries = Queries(
+            _canon_rows(ctx.gather_rows(base_lde, FP, N, nbase, positions), 1),
+            _canon_rows(ctx.gather_rows(ext_lde, fq, N, next_, positions), fq) if next_ else [],
+            _canon_rows(ctx.gather_rows(comp_lde, fq, N, ce_blowup, positions), fq),
+            self._view(base_tree, positions),
+            self._view(ext_tree, positions) if next_ else None,
+            self._view(comp_tree, positions))
+        return self._finish(r, fri_proof, queries)
+
+    # ---- streamed residency: coefficients and tree nodes stay, coset blocks are recomputed
+    def _commit_blocks(self, polys, blk, field, ncols, log_n, log_b, offsets):
+        """Merkle commitment of the bit-reversed LDE of `polys`, one coset block at a time: block q is transformed into
+        `blk` and hashed into its subtree of the node heap; the top log_b levels come from the block roots.
+        Returns (nodes, root)."""
+        ctx, beta = self.ctx, 1 << log_b
+        nodes, roots = self._empty(beta << log_n, 4), self._empty(beta, 4)
+        for q, h in offsets:
+            self._block(polys, blk, field, ncols, log_n, h)
+            ctx.merkle_commit_block(blk, field, log_n, log_b, q, ncols, nodes, roots[q])
+        if beta > 1:
+            ctx.merkle_nodes(roots, nodes, beta)
+        nodes[0].zero_()                        # the unused default digest (named by a walk over a 2-leaf tree)
+        return nodes, nodes[1].cpu().numpy().tobytes()
+
+    def _block(self, polys, blk, field, ncols, log_n, h):
+        """coset block with offset h of the bit-reversed LDE of every column of `polys`, into `blk`.  Its NTT plan is
+        dropped at once: every block has its own offset, and beta cached plans with their full tables (up to GiBs each
+        at 2^24 points) would take back the memory streaming saves"""
+        self.ctx.lde_batch(polys, blk, field, log_n, 0, ncols, offset=h, bitrev=True)
+        self.ctx.set_option("drop_plans", 1)
+
+    def _streamed_queries(self, polys, field, ncols, nodes, log_n, log_b, positions):
+        """the rows at `positions` and their MerkleView without the LDE: rows and leaf digests from the coefficients
+        (ms_lde_rows), path nodes gathered from the resident node heap"""
+        N = 1 << (log_n + log_b)
+        init, sib, path = merkle_walk(N, positions)
+        k = len(positions)
+        rows = self.ctx.lde_rows(polys, field, log_n, log_b, ncols, list(positions) + init + sib)
+
+        def leaf(row):                         # hash_rows: canonical words, 8 bytes little-endian each
+            return hashlib.sha256(b"".join((int(w) * _RINV % P).to_bytes(8, "little") for w in row)).digest()
+
+        digests = [leaf(row) for row in rows[k:]]
+        path_nodes = [d.tobytes() for d in self.ctx.gather_rows_rowmajor(nodes, 4, N, path)] if path else []
+        return rows[:k], MerkleView(path_nodes, digests[:len(init)], digests[len(init):], N.bit_length() - 1)
+
+    def _prove_streamed(self, r):
+        ctx, stark, trace, air, channel, lap = r.ctx, r.stark, r.trace, r.air, r.channel, r.lap
+        fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
+        offsets = coset_offsets(log_n, log_b)
+
+        # ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
+        host_base = trace.base_columns()
+        if tuple(host_base.shape) != (nbase, n):
+            raise ProvingError(f"expected {nbase} base columns of {n} rows")
+        base = self._to_device(host_base)
+        base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
+        ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
+        base_nodes, base_root = self._commit_blocks(base_polys, base_blk, FP, nbase, log_n, log_b, offsets)
+        channel.commit_base_trace(base_root)
+        lap("base_trace_commitment")
+        challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
+        hints = air.gen_hints(challenges)
+
+        # ---- extension trace commitment
+        ext = self._extension_columns(r, challenges, base)
+        del base
+        ext_polys = ext_blk = ext_nodes = None
+        if ext is not None:
+            ext_polys = self._empty(next_, n * fq)
+            ctx.ntt_batch_to(self._to_device(ext), ext_polys, fq, log_n, next_, inverse=True)
+            del ext
+            ext_blk = self._empty(next_, n * fq)
+            ext_nodes, ext_root = self._commit_blocks(ext_polys, ext_blk, fq, next_, log_n, log_b, offsets)
+            channel.commit_extension_trace(ext_root)
+        lap("extension_trace_commitment")
+
+        def trace_block(h):
+            self._block(base_polys, base_blk, FP, nbase, log_n, h)
+            cols = [base_blk[c] for c in range(nbase)]
+            if next_:
+                self._block(ext_polys, ext_blk, fq, next_, log_n, h)
+                cols += [ext_blk[c] for c in range(next_)]
+            return cols
+
+        # ---- constraint evaluation, block by block: the blocks q < ce_blowup of the LDE are the ce domain
+        ce_blowup = air.ce_blowup_factor
+        log_ce = log_n + ce_blowup.bit_length() - 1
+        M = n * ce_blowup
+        composition_coeffs = [channel.public_coin.draw() for _ in range(air.num_composition_constraint_coeffs())]
+        prog = block_program(r.cached_air).bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
+        comp_evals = self._empty(M * fq)
+        is_fq = [False] * nbase + [True] * next_
+        for q, h in offsets[:ce_blowup]:
+            ctx.eval_constraints_ptrs(prog, comp_evals[q * n * fq:(q + 1) * n * fq], log_n, trace_block(h), is_fq, fq_field=fq,
+                                      offset=h, trace_bitrev=True, out_bitrev=True)
+        lap("constraint_eval")
+
+        # ---- composition trace: the bit-reversed ce-domain column -> coefficients -> ce_blowup columns
+        ctx.bit_reverse(comp_evals, fq, log_ce)
+        ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
+        comp_polys = self._composition_columns(r, comp_evals)
+        del comp_evals                          # (when ce_blowup == 1, comp_polys is a view of it and keeps it)
+        ctx.set_option("drop_scratch", 1)       # the size-M transform's temporary: as large as the column itself
+        comp_blk = self._empty(ce_blowup, n * fq)
+        comp_nodes, comp_root = self._commit_blocks(comp_polys, comp_blk, fq, ce_blowup, log_n, log_b, offsets)
+        channel.commit_composition_trace(comp_root)
+        lap("composition_trace_commitment")
+
+        # ---- DEEP composition polynomial: every block of the three matrices recomputed once more
+        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
+        deep_lde = self._empty(N * fq)
+        is_fq = [False] * nbase + [True] * (next_ + ce_blowup)
+        for q, h in offsets:
+            cols = trace_block(h)
+            self._block(comp_polys, comp_blk, fq, ce_blowup, log_n, h)
+            cols += [comp_blk[c] for c in range(ce_blowup)]
+            ctx.eval_constraints_ptrs(dprog, deep_lde[q * n * fq:(q + 1) * n * fq], log_n, cols, is_fq, fq_field=fq, offset=h,
+                                      trace_bitrev=True, out_bitrev=True)
+        del base_blk, ext_blk, comp_blk
+        lap("deep_composition")
+
+        layers = self._fri(r, deep_lde)
+
+        # ---- queries: rows and leaf digests from the coefficients, path nodes from the node heaps
+        positions = channel.get_fri_query_positions()
+        fri_proof = self._fri_queries(r, layers, positions)
+        base_rows, base_view = self._streamed_queries(base_polys, FP, nbase, base_nodes, log_n, log_b, positions)
+        comp_rows, comp_view = self._streamed_queries(comp_polys, fq, ce_blowup, comp_nodes, log_n, log_b, positions)
+        ext_rows, ext_view = (self._streamed_queries(ext_polys, fq, next_, ext_nodes, log_n, log_b, positions) if next_
+                              else (None, None))
+        queries = Queries(_canon_rows(base_rows, 1), _canon_rows(ext_rows, fq) if next_ else [], _canon_rows(comp_rows, fq),
+                          base_view, ext_view, comp_view)
+        return self._finish(r, fri_proof, queries)
+
+    # ---- phases both residencies share
+    def _extension_columns(self, r, challenges, base):
+        if hasattr(r.trace, "build_extension_columns_device"):
+            # running products / evaluations as device scans over the resident base trace (SURVEY.md §8f rank 3)
+            ext = r.trace.build_extension_columns_device(challenges, r.ctx, base)
+        else:
+            ext = r.trace.build_extension_columns(challenges)
+        num_ext = 0 if ext is None else int(ext.shape[0])
+        if num_ext != r.next_:
+            raise ProvingError(f"expected {r.next_} extension columns, got {num_ext}")
+        return ext
+
+    def _composition_columns(self, r, comp_coeffs):
+        """the composition coefficients over the ce coset as ce_blowup columns, column i = coefficients = i mod ce_blowup"""
+        ce_blowup = r.air.ce_blowup_factor
+        if ce_blowup == 1:
+            return comp_coeffs.view(1, r.n * r.fq)
+        comp_polys = self._empty(ce_blowup, r.n * r.fq)
+        r.ctx.matrix_from_rows(comp_coeffs, comp_polys, r.fq, r.n, ce_blowup)
+        return comp_polys
+
+    def _bind_deep(self, r, base_polys, ext_polys, comp_polys):
+        """out-of-domain evaluations (composer.rs:43-86) from the coefficients, sent to the channel; then the DEEP
+        coefficients are drawn and bound into the DEEP program"""
+        ctx, air, channel, stark, fq, n = r.ctx, r.air, r.channel, r.stark, r.fq, r.n
+        nbase, next_, ce_blowup = r.nbase, r.next_, air.ce_blowup_factor
         z = channel.get_ood_point()
         zq = _lift(z)
         trace_arguments = air.trace_arguments()
         offsets = sorted(set(o for _, o in trace_arguments))
-        z_points, z_m = deep.ood_points(zq, log_n, offsets, ce_blowup)
+        z_points, z_m = deep.ood_points(zq, r.log_n, offsets, ce_blowup)
         pts = np.array([[_mont(c) for c in z_points[o]] for o in offsets], dtype=np.uint64).reshape(-1, 3)
         base_ood = ctx.poly_eval(base_polys, FP, n, nbase, pts)
         ext_ood = ctx.poly_eval(ext_polys, fq, n, next_, pts) if next_ else None
@@ -316,29 +557,21 @@ class GpuProver:
         composition_trace_oods = [unlift(comp_ood[j, 0]) for j in range(ce_blowup)]
         channel.send_ood_evals(execution_trace_oods, composition_trace_oods)
 
-        # ---- DEEP composition polynomial, evaluated straight over the LDE domain (composer.rs:89-188 in evaluation form)
         ex_alphas, co_alphas, (d_alpha, d_beta) = stark.gen_deep_coeffs(channel.public_coin, air)
         dprog_sym, dkeys = air.deep_program()
-        dprog = dprog_sym.bind(hints=deep.deep_hint_values(
+        return dprog_sym.bind(hints=deep.deep_hint_values(
             dkeys, z_points, z_m, [_lift(v) for v in execution_trace_oods], [_lift(v) for v in composition_trace_oods],
             [_lift(v) for v in ex_alphas], [_lift(v) for v in co_alphas], _lift(d_alpha), _lift(d_beta),
             trace_arguments=trace_arguments))
-        ncols_all = nbase + next_ + ce_blowup
-        sz = N * 8
-        cols = [base_lde.data_ptr() + c * sz for c in range(nbase)]
-        cols += [ext_lde.data_ptr() + c * sz * fq for c in range(next_)]
-        cols += [comp_lde.data_ptr() + c * sz * fq for c in range(ce_blowup)]
-        deep_lde = self._empty(N * fq)
-        ctx.eval_constraints_ptrs(dprog, deep_lde, log_N, cols, [False] * nbase + [True] * (ncols_all - nbase), fq_field=fq,
-                                  offset=GEN_MONT, trace_bitrev=True, out_bitrev=True)
-        lap("deep_composition")
 
-        # ---- FRI (fri.rs:179-249)
+    def _fri(self, r, deep_lde):
+        """FRI layers (fri.rs:179-249), the remainder and the proof of work; returns the committed layers"""
+        ctx, channel, options, fq, beta = r.ctx, r.channel, r.options, r.fq, r.beta
         ff = options.fri_folding_factor
         log_ff = ff.bit_length() - 1
         layers = []
-        cur, ln = deep_lde, log_N
-        for _ in range(options.fri_num_layers(N)):
+        cur, ln = deep_lde, r.log_N
+        for _ in range(options.fri_num_layers(r.N)):
             nrows = 1 << (ln - log_ff)
             leaves, nodes = self._empty(nrows, 4), self._empty(nrows, 4)
             root = ctx.merkle_commit_rows(cur, ff * fq, nrows, leaves=leaves, nodes=nodes)   # Matrix::from_arrays + from_matrix
@@ -362,28 +595,25 @@ class GpuProver:
         if any(c != zero for c in rem_coeffs[keep:]):
             raise ProvingError("FRI remainder is not low degree: the trace does not satisfy the AIR (fri.rs:246)")
         channel.commit_remainder(rem_coeffs[:keep])
-        lap("fri")
+        r.lap("fri")
 
         channel.grind_fri_commitments()
-        lap("proof_of_work")
+        r.lap("proof_of_work")
+        return layers
 
-        # ---- queries (fri.rs:151-177, trace.rs:115-157)
-        positions = channel.get_fri_query_positions()
+    def _fri_queries(self, r, layers, positions):
+        """FRI layer rows and paths at the folded query positions (fri.rs:151-177)"""
+        ff, fq = r.options.fri_folding_factor, r.fq
         fri_layers, folded = [], positions
         for evals, tree, root, nrows in layers:
             folded = sorted(set(p // ff for p in folded))                                    # fold_positions
-            rows = ctx.gather_rows_rowmajor(evals, ff * fq, nrows, folded)
+            rows = r.ctx.gather_rows_rowmajor(evals, ff * fq, nrows, folded)
             fri_layers.append(LayerProof(_canon_rows(rows, fq), self._view(tree, folded), root))
-        fri_proof = FriProof(fri_layers, channel.fri_remainder_coeffs)
-        queries = Queries(
-            _canon_rows(ctx.gather_rows(base_lde, FP, N, nbase, positions), 1),
-            _canon_rows(ctx.gather_rows(ext_lde, fq, N, next_, positions), fq) if next_ else [],
-            _canon_rows(ctx.gather_rows(comp_lde, fq, N, ce_blowup, positions), fq),
-            self._view(base_tree, positions),
-            self._view(ext_tree, positions) if next_ else None,
-            self._view(comp_tree, positions))
-        lap("queries")
-        timings["total"] = time.perf_counter() - t_all
-        return Proof(options, n, channel.base_trace_commitment, channel.extension_trace_commitment,
-                     channel.composition_trace_commitment, fri_proof, channel.pow_nonce, queries,
-                     channel.execution_trace_ood_evals, channel.composition_trace_ood_evals, timings)
+        return FriProof(fri_layers, r.channel.fri_remainder_coeffs)
+
+    def _finish(self, r, fri_proof, queries):
+        r.lap("queries")
+        r.timings["total"] = time.perf_counter() - r.t_all
+        c = r.channel
+        return Proof(r.options, r.n, c.base_trace_commitment, c.extension_trace_commitment, c.composition_trace_commitment,
+                     fri_proof, c.pow_nonce, queries, c.execution_trace_ood_evals, c.composition_trace_ood_evals, r.timings)

@@ -34,49 +34,13 @@ from . import deep
 from . import expr as E
 from .air import domain_generator
 from .channel import ProverChannel
+from .cosets import block_program, brev as _brev, coset_offsets, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
 from .prover import GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont
 
 P = E.P
 _R = 2**64
 _RINV = pow(_R, -1, P)
-
-
-def _brev(v, bits):
-    r = 0
-    for _ in range(bits):
-        r = (r << 1) | (v & 1)
-        v >>= 1
-    return r
-
-
-def merkle_walk(n_leaves, indices):
-    """The index walk of MerkleTreeImpl::prove (src/merkle.rs:149-207; csrc/hash.cu ms_merkle_prove_sha256): which
-    leaves and which heap nodes a batched proof names.  Returns (initial leaf indices, sibling leaf indices, node indices)."""
-    idx = sorted(set(int(i) for i in indices))
-    init, sib, path, node_q = [], [], [], []
-    k = 0
-    while k < len(idx):
-        i = idx[k]
-        init.append(i)
-        node_q.append((n_leaves + i) >> 1)
-        if k + 1 < len(idx) and (i ^ 1) == idx[k + 1]:
-            init.append(idx[k + 1])
-            k += 2
-            continue
-        sib.append(i ^ 1)
-        k += 1
-    head = 0
-    while head < len(node_q):
-        i = node_q[head]
-        head += 1
-        if i > 2:
-            node_q.append(i >> 1)
-        if head < len(node_q) and (i ^ 1) == node_q[head]:
-            head += 1
-            continue
-        path.append(i ^ 1)
-    return init, sib, path
 
 
 def top_levels(sub_roots):
@@ -252,9 +216,8 @@ class ShardedProver(GpuProver):
 
     def _offsets(self, log_n, log_b):
         """Montgomery words of h_q = offset * g_N^bitrev(q) for this rank's blocks"""
-        gN = domain_generator(log_n + log_b)
         bpr = (1 << log_b) // self.world
-        return [(q, 7 * pow(gN, _brev(q, log_b), P) % P * _R % P) for q in range(self.rank * bpr, (self.rank + 1) * bpr)]
+        return coset_offsets(log_n, log_b, range(self.rank * bpr, (self.rank + 1) * bpr))
 
     def _lde_slab(self, polys, field, ncols, log_n, log_b):
         """this rank's blocks of the bit-reversed LDE of every column: (ncols, N/G) elements, block j at rows [j n, (j+1) n)"""
@@ -355,9 +318,7 @@ class ShardedProver(GpuProver):
             air0 = Air(cfg, n, None, options)
             air0.composition_program()
             air0.deep_program()
-            # the composition evaluated block by block: inside a block the ce-domain stride is 1 and the domain has n points
-            air0._block_program = E.compile_program(air0.composition_constraint, cfg.NUM_BASE_COLUMNS, lde_step=1,
-                                                    log_ce=air0.log_n, symbolic=True, batch_inverses=True)
+            block_program(air0)              # the composition evaluated block by block
             air0.num_challenges(), air0.num_composition_constraint_coeffs(), air0.trace_arguments()
             self._airs[key] = air0
         air = copy.copy(self._airs[key])
