@@ -297,6 +297,21 @@ class Context:
                                                    program.consts.ctypes.data, program.consts.shape[0], ptrs, isq, k,
                                                    fq_field, log_m, offset, int(trace_bitrev), int(out_bitrev), _ptr(out)))
 
+    def check_constraints(self, program, cols, cols_are_fq, fq_field, log_n, nconstraints):
+        """Constraint::check (src/constraints.rs:168-249) of constraints 0..nconstraints-1 of a checked `program`
+        (expr.compile_check_program, bound) at every row of the trace domain 2^log_n; `cols`: natural-order device
+        columns, then the program's periodic tables.  Returns (first_row, fail_count), numpy uint64 arrays of
+        nconstraints: the lowest failing row (2^64 - 1 where none fails) and the number of failing rows."""
+        k = len(cols)
+        ptrs = (C.c_void_p * max(k, 1))(*[_ptr(c) for c in cols])
+        isq = (C.c_int * max(k, 1))(*[int(bool(q)) for q in cols_are_fq])
+        first_row = np.empty(nconstraints, dtype=np.uint64)
+        fail_count = np.empty(nconstraints, dtype=np.uint64)
+        self._ck(self.lib.ms_check_constraints(self.h, program.code.ctypes.data, len(program), program.consts.ctypes.data,
+                                               program.consts.shape[0], ptrs, isq, k, fq_field, log_n, nconstraints,
+                                               first_row.ctypes.data, fail_count.ctypes.data))
+        return first_row, fail_count
+
     def poly_eval(self, coeffs, field, n, ncols, points, col_stride=None):
         """horner_evaluate of every column at every point (get_ood_evals, src/composer.rs:43-86).
         points: (k, 3) Montgomery words; returns (ncols, k, 3) numpy uint64."""

@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MS_LIB_PATH") or os.path.join(_HERE, "libministark_b200.so")   # MS_LIB_PATH: A/B builds
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h")
 STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
+CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -71,6 +72,11 @@ _STREAM_SIGS = {
     "ms_lde_rows": (ci, [vp, ci, vp, sz, ui, ui, ui, u64, vp, ui, vp]),
 }
 
+# include/ministark_check.h: the constraint check behind the prover's optional validation (validate.py)
+_CHECK_SIGS = {
+    "ms_check_constraints": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ci, ui, ui, vp, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -99,6 +105,7 @@ def load():
         lib = C.CDLL(LIB_PATH)
         bind(lib, _SIGS)
         bind(lib, _STREAM_SIGS)
+        bind(lib, _CHECK_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

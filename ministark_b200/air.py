@@ -212,6 +212,15 @@ class Air:
                                                     batch_inverses=True), keys)
         return self._deep_program
 
+    def check_program(self):
+        """every constraint as one checked program over the trace domain (csrc/check.cu; challenges and hints are bound
+        per proof), for the prover's optional constraint validation (ministark_b200/validate.py)"""
+        if getattr(self, "_check_program", None) is None:
+            cfg = self.config
+            self._check_program = E.compile_check_program(self.constraints, cfg.NUM_BASE_COLUMNS, self.log_n,
+                                                          cfg.NUM_BASE_COLUMNS + cfg.NUM_EXTENSION_COLUMNS)
+        return self._check_program
+
     # the three walks below depend on the constraints only: done once per Air (the provers copy a cached Air per proof,
     # and each walk of the brainfuck AIR costs ~0.5 ms of a 10 ms proof)
     def num_challenges(self):

@@ -22,14 +22,11 @@
 //    coalesced and neither CPU permutation is needed.
 //  * Div is a per-point field inversion (Fermat chain); eval_cpu uses batch inversion per chunk
 //    (eval_cpu.rs:280-295) — the same field element either way.
-#include "ctx.cuh"
+#include "eval.cuh"
 
 namespace ms {
 
 using gl::Fq3;
-
-enum { OP_X = 0, OP_CONST, OP_TRACE, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_INV, OP_POW, OP_STORE, OP_PERIODIC };
-constexpr int kMaxRegs = 48;
 
 struct EvalParams {
     const uint4 *prog;
@@ -179,6 +176,44 @@ __global__ void __launch_bounds__(128) eval_kernel(const EvalParams p) {
     }
 }
 
+int validate_program(ms_ctx *c, const char *who, const uint32_t *program, unsigned nprog, unsigned nconsts,
+                     const std::vector<int> &col_is_q, unsigned log_m, unsigned nconstraints) {
+    const bool checked = nconstraints > 0;
+    std::vector<char> defined(kMaxRegs, 0);
+    bool stored = false;
+    for (unsigned k = 0; k < nprog; k++) {
+        const uint32_t *ins = program + 4 * k;
+        const uint32_t op = ins[0] & 0xff;
+        if (op > (checked ? (uint32_t)OP_CHECK : (uint32_t)OP_PERIODIC) || ins[1] >= (uint32_t)kMaxRegs)
+            return fail(c, MS_ERR_INVALID, "%s: bad instruction %u", who, k);
+        if (checked && (op == OP_STORE || op == OP_INV))
+            return fail(c, MS_ERR_INVALID, "%s: instruction %u: %s has no place in a checked program", who, k, op == OP_STORE ? "STORE" : "INV");
+        if (op == OP_CONST && ins[2] >= nconsts) return fail(c, MS_ERR_INVALID, "%s: constant index out of range", who);
+        if (op == OP_TRACE || op == OP_PERIODIC) {
+            const int is_q = (ins[0] >> 8) & 1;
+            if (ins[2] >= col_is_q.size()) return fail(c, MS_ERR_INVALID, "%s: column %u out of range", who, ins[2]);
+            if (col_is_q[ins[2]] != is_q) return fail(c, MS_ERR_INVALID, "%s: column %u has the wrong field", who, ins[2]);
+            if (op == OP_PERIODIC && ins[3] > log_m) return fail(c, MS_ERR_INVALID, "%s: periodic table longer than the domain", who);
+        }
+        if (op == OP_CHECK && ins[3] >= nconstraints)
+            return fail(c, MS_ERR_INVALID, "%s: instruction %u checks constraint %u of %u", who, k, ins[3], nconstraints);
+        const bool unary = op == OP_NEG || op == OP_INV || op == OP_POW || op == OP_STORE || op == OP_CHECK;
+        const bool binary = op == OP_ADD || op == OP_SUB || op == OP_MUL || op == OP_DIV;
+        if (unary || binary) {
+            if (ins[2] >= (uint32_t)kMaxRegs || !defined[ins[2]])
+                return fail(c, MS_ERR_INVALID, "%s: instruction %u reads register %u before it is written", who, k, ins[2]);
+        }
+        if (binary) {
+            if (ins[3] >= (uint32_t)kMaxRegs || !defined[ins[3]])
+                return fail(c, MS_ERR_INVALID, "%s: instruction %u reads register %u before it is written", who, k, ins[3]);
+        }
+        if (op == OP_STORE) stored = true;
+        else if (op != OP_CHECK) defined[ins[1]] = 1;
+    }
+    if (!checked && !stored) return fail(c, MS_ERR_INVALID, "%s: program stores no result", who);
+    return MS_OK;
+}
+
 int eval_launch_jit(ms_ctx *c, const uint32_t *program, unsigned nprog, const uint64_t *consts, unsigned nconsts,
                     const u64 *const *dev_col_ptr, const u64 *dev_consts, int fq_field, unsigned log_m, uint64_t offset_mont,
                     int trace_bitrev, int out_bitrev, const u64 *tw_lo, const u64 *tw_hi, u32 hi_len, u64 *out_dev);
@@ -191,41 +226,12 @@ static int eval_launch(ms_ctx *c, const uint32_t *program, unsigned nprog, const
                        const std::vector<const u64 *> &cols, const std::vector<int> &col_is_q, int fq_field, unsigned log_m,
                        uint64_t offset_mont, int trace_bitrev, int out_bitrev, u64 *out_dev) {
     const size_t M = (size_t)1 << log_m;
-    // validate the program against the register file, constant pool and column table; every source register must
-    // have been written by an earlier instruction
-    {
-        std::vector<char> defined(kMaxRegs, 0);
-        bool stored = false;
-        for (unsigned k = 0; k < nprog; k++) {
-            const uint32_t *ins = program + 4 * k;
-            const uint32_t op = ins[0] & 0xff;
-            if (op > OP_PERIODIC || ins[1] >= (uint32_t)kMaxRegs) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: bad instruction %u", k);
-            if (op == OP_CONST && ins[2] >= nconsts) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: constant index out of range");
-            if (op == OP_TRACE || op == OP_PERIODIC) {
-                const int is_q = (ins[0] >> 8) & 1;
-                if (ins[2] >= cols.size()) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: column %u out of range", ins[2]);
-                if (col_is_q[ins[2]] != is_q) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: column %u has the wrong field", ins[2]);
-                if (op == OP_PERIODIC && ins[3] > log_m) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: periodic table longer than the domain");
-            }
-            const bool unary = op == OP_NEG || op == OP_INV || op == OP_POW || op == OP_STORE;
-            const bool binary = op == OP_ADD || op == OP_SUB || op == OP_MUL;
-            if (unary || binary) {
-                if (ins[2] >= (uint32_t)kMaxRegs || !defined[ins[2]])
-                    return fail(c, MS_ERR_INVALID, "ms_eval_constraints: instruction %u reads register %u before it is written", k, ins[2]);
-            }
-            if (binary) {
-                if (ins[3] >= (uint32_t)kMaxRegs || !defined[ins[3]])
-                    return fail(c, MS_ERR_INVALID, "ms_eval_constraints: instruction %u reads register %u before it is written", k, ins[3]);
-            }
-            if (op == OP_STORE) stored = true;
-            else defined[ins[1]] = 1;
-        }
-        if (!stored) return fail(c, MS_ERR_INVALID, "ms_eval_constraints: program stores no result");
-    }
+    int rc = validate_program(c, "ms_eval_constraints", program, nprog, nconsts, col_is_q, log_m, 0);
+    if (rc) return rc;
     // program, constants and the column pointer table are tiny: always copied to the device
     void *meta;
     const size_t prog_bytes = (size_t)nprog * 16, const_bytes = (size_t)nconsts * 24, ptr_bytes = cols.size() * 8;
-    int rc = scratch_get(c, 3, prog_bytes + const_bytes + ptr_bytes + 64, &meta);
+    rc = scratch_get(c, 3, prog_bytes + const_bytes + ptr_bytes + 64, &meta);
     if (rc) return rc;
     MS_CUDA(c, cudaMemcpyAsync(meta, program, prog_bytes, cudaMemcpyDefault, c->stream));
     MS_CUDA(c, cudaMemcpyAsync((char *)meta + prog_bytes, consts, const_bytes, cudaMemcpyDefault, c->stream));

@@ -21,8 +21,9 @@ _RINV = pow(_R, -1, P)
 
 FP, FQ = 0, 1  # value types: base field / extension ("Fq" is Fq3, or Fp itself when the AIR has Fq = Fp)
 
-# opcodes (must match csrc/eval.cu)
-OP_X, OP_CONST, OP_TRACE, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_INV, OP_POW, OP_STORE, OP_PERIODIC = range(11)
+# opcodes (must match csrc/eval.cuh).  OP_DIV and OP_CHECK occur only in checked programs (compile_check_program,
+# csrc/check.cu): OP_DIV is Constraint::check's division, OP_CHECK k, r marks constraint k failed where register r is None
+OP_X, OP_CONST, OP_TRACE, OP_NEG, OP_ADD, OP_SUB, OP_MUL, OP_INV, OP_POW, OP_STORE, OP_PERIODIC, OP_DIV, OP_CHECK = range(13)
 MAX_REGS = 48
 
 
@@ -290,37 +291,7 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
     base-field column, otherwise extension column col - num_base_cols; the row shift is
     lde_step * off (eval_cpu.rs:119-123).  The result is always stored as an Fq element.
     """
-    order, seen = [], set()
     trace_len = (1 << log_ce) // lde_step if log_ce is not None and lde_step >= 1 else 0
-
-    def visit(e):                      # iterative post-order (DAGs can be deep)
-        # Sethi-Ullman flavoured order: the operand with the larger subtree is evaluated first, so a long
-        # left-deep sum of constraint terms keeps one accumulator live instead of every term
-        size, st = {}, [(e, False)]
-        while st:
-            node, done = st.pop()
-            if done:
-                size[id(node)] = 1 + sum(size[id(a)] for a in node.args if isinstance(a, Expr))
-                continue
-            if id(node) in size:
-                continue
-            size[id(node)] = 0
-            st.append((node, True))
-            st.extend((a, False) for a in node.args if isinstance(a, Expr) and id(a) not in size)
-        stack = [(e, False)]
-        while stack:
-            node, done = stack.pop()
-            if id(node) in seen and not done:
-                continue
-            if done:
-                order.append(node)
-                continue
-            seen.add(id(node))
-            stack.append((node, True))
-            kids = [a for a in node.args if isinstance(a, Expr) and id(a) not in seen]
-            kids.sort(key=lambda a: size[id(a)])          # popped last-in first-out: largest subtree first
-            for a in kids:
-                stack.append((a, False))
 
     # a / b  ->  a * inv(b) with inv(b) hash-consed, so a denominator shared by many constraints
     # (the zerofier X^n - 1) is inverted once per point instead of once per Div node
@@ -358,7 +329,65 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
     expr = rewrite(expr)
     if batch_inverses:
         expr = _batch_inverses(expr, num_base_cols)
-    visit(expr)
+    code, consts, nregs, typ, bindings, periodic = _lower(
+        [expr], lambda k, r, t: [OP_STORE | (t << 8), 0, r, 0], num_base_cols, challenges, hints, lde_step, log_ce, symbolic,
+        num_cols, max_live_leaves)
+    return Program(code, consts, nregs, typ[id(expr)] == FQ, bindings, periodic)
+
+
+def compile_check_program(constraints, num_base_cols, log_n, num_cols, symbolic=True, challenges=(), hints=()):
+    """Flatten every constraint into ONE checked program for csrc/check.cu, which runs Constraint::check
+    (src/constraints.rs:168-249) at every row of the trace domain of size 2^log_n: values carry a None flag, Div is the
+    checked division (OP_DIV) and root k ends with OP_CHECK k.  Subexpressions shared by several constraints (x^n - 1,
+    a transition term) are hash-consed and computed once per row.
+
+    Unlike compile_program: no a/b -> a * inv(b) rewrite and no batched inverses (a vanishing denominator is exactly
+    what the check looks for), and a division whose denominator folds to zero on the host is left to the kernel, so
+    host folding gives the kernel's Option result.  Trace(col, off) reads column[(i + off) mod 2^log_n]; periodic
+    tables come from periodic_tables(ctx, program, log_n, 1, offset_canonical=1)."""
+    roots = list(constraints)
+    code, consts, nregs, _, bindings, periodic = _lower(
+        roots, lambda k, r, t: [OP_CHECK, 0, r, k], num_base_cols, challenges, hints, 1, log_n, symbolic, num_cols, None)
+    return Program(code, consts, nregs, False, bindings, periodic)
+
+
+def _lower(roots, finish, num_base_cols, challenges, hints, lde_step, log_ce, symbolic, num_cols, max_live_leaves):
+    """post-order, constant folding, typing and register allocation of the DAG under `roots`; finish(k, register, type)
+    gives the instruction that consumes root k right after it is computed.  Returns (code, consts, nregs, typ,
+    bindings, periodic)."""
+    order, seen = [], set()
+
+    def visit(e):                      # iterative post-order (DAGs can be deep)
+        # Sethi-Ullman flavoured order: the operand with the larger subtree is evaluated first, so a long
+        # left-deep sum of constraint terms keeps one accumulator live instead of every term
+        size, st = {}, [(e, False)]
+        while st:
+            node, done = st.pop()
+            if done:
+                size[id(node)] = 1 + sum(size[id(a)] for a in node.args if isinstance(a, Expr))
+                continue
+            if id(node) in size:
+                continue
+            size[id(node)] = 0
+            st.append((node, True))
+            st.extend((a, False) for a in node.args if isinstance(a, Expr) and id(a) not in size)
+        stack = [(e, False)]
+        while stack:
+            node, done = stack.pop()
+            if id(node) in seen and not done:
+                continue
+            if done:
+                order.append(node)
+                continue
+            seen.add(id(node))
+            stack.append((node, True))
+            kids = [a for a in node.args if isinstance(a, Expr) and id(a) not in seen]
+            kids.sort(key=lambda a: size[id(a)])          # popped last-in first-out: largest subtree first
+            for a in kids:
+                stack.append((a, False))
+
+    for e in roots:
+        visit(e)
     # constant folding + typing
     cval, typ = {}, {}
     for nd in order:
@@ -395,8 +424,13 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
                     cval[id(nd)] = q_inv(v[0])
                 elif k == "pow":
                     cval[id(nd)] = q_pow(v[0], a[1])
+                elif k == "div" and any(v[1]):
+                    cval[id(nd)] = q_mul(v[0], q_inv(v[1]))     # a zero denominator is left to the checked kernel
+    root_of = {}
+    for i, e in enumerate(roots):
+        root_of.setdefault(id(e), []).append(i)
     # last use (for register reuse), skipping folded nodes
-    live_nodes = [nd for nd in order if id(nd) not in cval or nd is expr]
+    live_nodes = [nd for nd in order if id(nd) not in cval or id(nd) in root_of]
     last_use = {}
     for idx, nd in enumerate(live_nodes):
         for x in nd.args:
@@ -491,24 +525,32 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
             free.append(reg_of.pop(id(x)))
             leaf_regs.pop(id(x), None)
 
+    def finish_roots(nd, idx):
+        for i in root_of.get(id(nd), ()):
+            code.append(finish(i, reg_of[id(nd)], typ[id(nd)]))
+        if last_use.get(id(nd), -1) <= idx and id(nd) in reg_of:     # no later consumer: the register is free again
+            free.append(reg_of.pop(id(nd)))
+            leaf_regs.pop(id(nd), None)
+
     for idx, nd in enumerate(live_nodes):
         k, a = nd.kind, nd.args
         pinned.clear()
         if is_leaf(nd):
-            if nd is expr:            # the root itself is a leaf / constant
+            if id(nd) in root_of:     # a root that is itself a leaf / constant
                 operand(nd)
+                finish_roots(nd, idx)
             continue                  # loaded lazily at first use
         if k == "neg":
             ra = operand(a[0])
             release(a[0], idx)
             r = alloc()
             code.append([OP_NEG | (typ[id(a[0])] << 8), r, ra, 0])
-        elif k in ("add", "mul"):
+        elif k in ("add", "mul", "div"):
             ra, rb = operand(a[0]), operand(a[1])
             release(a[0], idx)
             release(a[1], idx)
             r = alloc()
-            op = OP_ADD if k == "add" else OP_MUL
+            op = {"add": OP_ADD, "mul": OP_MUL, "div": OP_DIV}[k]
             code.append([op | (typ[id(a[0])] << 8) | (typ[id(a[1])] << 9), r, ra, rb])
         elif k == "inv":
             ra = operand(a[0])
@@ -525,6 +567,7 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
         else:
             raise ValueError(f"unsupported node {k}")
         reg_of[id(nd)] = r
-    code.append([OP_STORE | (typ[id(expr)] << 8), 0, reg_of[id(expr)], 0])
-    return Program(np.array(code, dtype=np.uint32), np.array(consts if consts else [[0, 0, 0]], dtype=np.uint64),
-                   max(nregs, 1), typ[id(expr)] == FQ, bindings, periodic)
+        if id(nd) in root_of:
+            finish_roots(nd, idx)
+    return (np.array(code, dtype=np.uint32), np.array(consts if consts else [[0, 0, 0]], dtype=np.uint64), max(nregs, 1), typ,
+            bindings, periodic)

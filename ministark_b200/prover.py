@@ -111,10 +111,20 @@ class Stark:
         co = [public_coin.draw() for _ in range(air.ce_blowup_factor)]
         return ex, co, (public_coin.draw(), public_coin.draw())
 
-    def prove(self, options, witness, device=0):
+    def prove(self, options, witness, device=0, validate=False):
         """Stark::prove (src/stark.rs:57-63).  The per-device prover (context, stream, compiled AIR programs) is created
-        on first use and reused, like the reference's process-global Planner."""
-        return GpuProver.shared(device).prove(self, options, witness)
+        on first use and reused, like the reference's process-global Planner.  validate=True: check the trace against
+        the AIR before the composition polynomial is computed (validate_constraints)."""
+        return GpuProver.shared(device).prove(self, options, witness, validate=validate)
+
+    def validate_constraints(self, air, challenges, hints, base_trace, extension_trace, ctx):
+        """Stark::validate_constraints (src/stark.rs:65-75), called by `prove(..., validate=True)` right after the
+        extension trace commitment (src/prover.rs:74-75) with the natural-order base and extension columns on the device.
+        Default: every constraint at every row (ministark_b200/validate.py); raises ConstraintViolation if any fails."""
+        from .validate import ConstraintViolation, validate_constraints
+        violations = validate_constraints(ctx, air, challenges, hints, base_trace, extension_trace)
+        if violations:
+            raise ConstraintViolation(violations)
 
 
 # Device memory torch does not see, kept free on top of either estimate: the NTT plans with their twiddle and scale
@@ -228,11 +238,17 @@ class GpuProver:
                            f"{_gib(est['streamed'])} streamed, and {_gib(budget)} is available")
 
     # ---- default_prove
-    def prove(self, stark, options, witness):
+    def prove(self, stark, options, witness, validate=False):
+        """default_prove.  validate=True: stark.validate_constraints checks the trace against the AIR once the extension
+        trace is committed, and raises before anything after that commitment is computed; its time is recorded as
+        timings["validate_constraints"].  The proof bytes do not depend on it.  (ShardedProver, whose ranks may not hold
+        the whole base trace, does not take it.)"""
         with torch.cuda.stream(self.stream):
+            if validate:
+                return self._prove(stark, options, witness, validate=True)
             return self._prove(stark, options, witness)
 
-    def _prove(self, stark, options, witness):
+    def _prove(self, stark, options, witness, validate=False):
         ctx = self.ctx
         cfg = stark.AirConfig
         timings = {}
@@ -250,6 +266,8 @@ class GpuProver:
             t = time.perf_counter()
             timings[name] = t - t0
             t0 = t
+            if name not in phases:          # validate_constraints: timed, outside the fixed phases
+                return
             torch.cuda.nvtx.range_pop()
             k = phases.index(name) + 1
             if k < len(phases):
@@ -277,7 +295,7 @@ class GpuProver:
         channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
         r = _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
                  beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
-                 timings=timings, t_all=t_all, cached_air=self._airs[key])
+                 timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate)
         lap("init_air")
         return self._prove_resident(r) if residency == "resident" else self._prove_streamed(r)
 
@@ -322,13 +340,17 @@ class GpuProver:
 
         # ---- extension trace commitment (prover.rs:56-72)
         ext = self._extension_columns(r, challenges, base)
+        check = self._keep_for_check(r, base, ext)
         del base
         ext_polys = ext_lde = ext_tree = None
         if ext is not None:
+            ext = check[1] if check else ext           # with validation: the one device copy serves both
             ext_polys, ext_lde, ext_tree, ext_root = self._commit_columns(self._to_device(ext), fq, log_n, log_b, next_, True)
             channel.commit_extension_trace(ext_root)
         del ext
         lap("extension_trace_commitment")
+        self._check(r, challenges, hints, check)
+        del check
 
         # ---- constraint evaluation over the ce domain (prover.rs:75-108).  The first M entries of a bit-reversed LDE
         # column ARE the ce-coset evaluations in bit-reversed order, so they are read in place (trace_bitrev).
@@ -432,9 +454,11 @@ class GpuProver:
 
         # ---- extension trace commitment
         ext = self._extension_columns(r, challenges, base)
+        check = self._keep_for_check(r, base, ext)
         del base
         ext_polys = ext_blk = ext_nodes = None
         if ext is not None:
+            ext = check[1] if check else ext
             ext_polys = self._empty(next_, n * fq)
             ctx.ntt_batch_to(self._to_device(ext), ext_polys, fq, log_n, next_, inverse=True)
             del ext
@@ -442,6 +466,8 @@ class GpuProver:
             ext_nodes, ext_root = self._commit_blocks(ext_polys, ext_blk, fq, next_, log_n, log_b, offsets)
             channel.commit_extension_trace(ext_root)
         lap("extension_trace_commitment")
+        self._check(r, challenges, hints, check)
+        del check
 
         def trace_block(h):
             self._block(base_polys, base_blk, FP, nbase, log_n, h)
@@ -502,6 +528,20 @@ class GpuProver:
         return self._finish(r, fri_proof, queries)
 
     # ---- phases both residencies share
+    def _keep_for_check(self, r, base, ext):
+        """with validation: the natural-order base columns and the extension columns on the device (a host-built
+        extension matrix uploaded once, for the check and the commitment), kept until the check has run"""
+        if not r.validate:
+            return None
+        return base, None if ext is None else self._to_device(ext)
+
+    def _check(self, r, challenges, hints, check):
+        """Stark::validate_constraints at the reference's position (src/prover.rs:74-75)"""
+        if check is not None:
+            r.air._check_program = r.cached_air.check_program()      # compiled once per AIR and trace length
+            r.stark.validate_constraints(r.air, challenges, hints, check[0], check[1], r.ctx)
+            r.lap("validate_constraints")
+
     def _extension_columns(self, r, challenges, base):
         if hasattr(r.trace, "build_extension_columns_device"):
             # running products / evaluations as device scans over the resident base trace (SURVEY.md §8f rank 3)
