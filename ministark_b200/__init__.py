@@ -324,6 +324,46 @@ class Context:
     def fill_random(self, dst, nwords, seed):
         self._ck(self.lib.ms_fill_random(self.h, _ptr(dst), nwords, seed))
 
+    # ---- examples/brainfuck execution trace (include/ministark_bf.h)
+    def bf_trace_sizes(self, program, program_len, log, nrec):
+        """table lengths of the trace of a run (ms_bf_trace_sizes): dict with proc_rows, instr_rows, mem_rows, reads,
+        writes, n and work_bytes (the workspace bf_trace_fill needs).  program: uint32 words; log: nrec records"""
+        s = np.zeros(len(BF_SIZES), dtype=np.uint64)
+        self._ck(self.lib.ms_bf_trace_sizes(self.h, _ptr(program), program_len, _ptr(log), nrec, s.ctypes.data))
+        return dict(zip(BF_SIZES, (int(v) for v in s)))
+
+    def bf_trace_fill(self, program, program_len, log, nrec, sizes, work, out):
+        """fill `out`, the (17, n) base matrix, from the same program and log (ms_bf_trace_fill); work: device buffer of
+        sizes["work_bytes"] bytes"""
+        s = np.array([sizes[k] for k in BF_SIZES], dtype=np.uint64)
+        self._ck(self.lib.ms_bf_trace_fill(self.h, _ptr(program), program_len, _ptr(log), nrec, s.ctypes.data, _ptr(work),
+                                           _ptr(out)))
+
+    def bf_helper_columns(self, base, n, aux):
+        """the eight helper columns of BrainfuckTrace.helper_columns() from a (17, n) base matrix into (8, n) `aux`"""
+        self._ck(self.lib.ms_bf_helper_columns(self.h, _ptr(base), n, _ptr(aux)))
+
+
+BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
+
+
+def bf_run(program, input_bytes=b"", max_cycles=1 << 26):
+    """ms_bf_run: the brainfuck VM over a compiled program (uint32 words) on the host.  Returns (log, output bytes): the
+    uint64 records of the cycles + 1 processor rows (include/ministark_bf.h).  Raises MsError when the memory pointer
+    leaves the tape, the input runs out or max_cycles cycles do not reach the end of the program."""
+    lib = _lib.load()
+    prog = np.ascontiguousarray(program, dtype=np.uint32)
+    inp = np.frombuffer(bytes(input_bytes), dtype=np.uint8).copy()
+    log = np.empty(max_cycles + 1, dtype=np.uint64)         # pages the run does not reach are never touched
+    out = np.empty(max(max_cycles, 1), dtype=np.uint8)
+    counts = np.zeros(2, dtype=np.uint64)
+    rc = lib.ms_bf_run(prog.ctypes.data, prog.size, inp.ctypes.data, inp.size, max_cycles, log.ctypes.data,
+                       out.ctypes.data, counts.ctypes.data)
+    if rc != 0:
+        raise MsError(f"[{rc}] {lib.ms_last_error(None).decode()}")
+    cycles, nout = int(counts[0]), int(counts[1])
+    return log[:cycles + 1].copy(), out[:nout].tobytes()
+
 
 _default_ctx = None
 

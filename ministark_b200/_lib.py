@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("MS_LIB_PATH") or os.path.join(_HERE, "libministark_b2
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h")
 STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
+BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -77,6 +78,14 @@ _CHECK_SIGS = {
     "ms_check_constraints": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ci, ui, ui, vp, vp]),
 }
 
+# include/ministark_bf.h: the execution trace of examples/brainfuck (VM on the host, tables on the device)
+_BF_SIGS = {
+    "ms_bf_run": (ci, [vp, sz, vp, sz, u64, vp, vp, vp]),
+    "ms_bf_trace_sizes": (ci, [vp, vp, sz, vp, sz, vp]),
+    "ms_bf_trace_fill": (ci, [vp, vp, sz, vp, sz, vp, vp, vp]),
+    "ms_bf_helper_columns": (ci, [vp, vp, sz, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -106,6 +115,7 @@ def load():
         bind(lib, _SIGS)
         bind(lib, _STREAM_SIGS)
         bind(lib, _CHECK_SIGS)
+        bind(lib, _BF_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -15,6 +15,21 @@ int fail(ms_ctx *c, int code, const char *fmt, ...) {
     return code;
 }
 
+// the message of the context-free entry point ms_bf_run on this thread, if its last call failed: ms_last_error(NULL)
+static thread_local std::string t_noctx_err;
+
+int fail_noctx(int code, const char *fmt, ...) {
+    char buf[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    va_end(ap);
+    t_noctx_err = buf;
+    return code;
+}
+
+void clear_noctx_error() { t_noctx_err.clear(); }
+
 int scratch_get(ms_ctx *c, int slot, size_t bytes, void **out) {
     Scratch &s = c->scratch[slot];
     if (s.cap < bytes) {
@@ -242,7 +257,7 @@ int ms_set_option(ms_ctx *c, const char *name, int64_t value) {
     return fail(c, MS_ERR_INVALID, "unknown option %s", name);
 }
 
-const char *ms_last_error(ms_ctx *c) { return c ? c->err.c_str() : "null context"; }
+const char *ms_last_error(ms_ctx *c) { return c ? c->err.c_str() : t_noctx_err.empty() ? "null context" : t_noctx_err.c_str(); }
 uint64_t ms_launch_count(ms_ctx *c) { return c ? c->launches : 0; }
 
 int ms_alloc_device(ms_ctx *c, size_t bytes, void **out) {

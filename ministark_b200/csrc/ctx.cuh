@@ -54,6 +54,9 @@ struct ms_ctx {
 namespace ms {
 
 int fail(ms_ctx *c, int code, const char *fmt, ...);
+// failures of ms_bf_run, which takes no context: the message is ms_last_error(NULL) until the thread's next ms_bf_run
+int fail_noctx(int code, const char *fmt, ...);
+void clear_noctx_error();
 #define MS_CUDA(ctx, expr)                                                                          \
     do {                                                                                            \
         cudaError_t _e = (expr);                                                                    \

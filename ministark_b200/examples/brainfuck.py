@@ -70,8 +70,14 @@ def compile_program(source):
     return program
 
 
-def simulate(source, input_bytes=b""):
-    """returns (BrainfuckTrace, output bytes)"""
+def simulate(source, input_bytes=b"", device=None, max_cycles=1 << 26):
+    """returns (BrainfuckTrace, output bytes).
+    device: run the VM natively (ms_bf_run) and build every table ON that device instead: returns
+    (BrainfuckDeviceTrace, output bytes), whose base_columns() is the resident (17, n) tensor, identical word for word to
+    the host trace's.  Raises MsError, before anything of the trace's size is allocated, when the memory pointer leaves
+    the 1024-cell tape, the input runs out, or max_cycles cycles do not end the program."""
+    if device is not None:
+        return _simulate_device(source, input_bytes, device, max_cycles)
     program = compile_program(source)
     get = lambda i: program[i] if i < len(program) else 0
     tape = [0] * 1024
@@ -227,7 +233,9 @@ class BrainfuckTrace(Trace):
         return self._aux
 
     def build_extension_columns_device(self, challenges, ctx, base_dev):
-        return _device_extension(self, [tuple(c) for c in challenges], ctx, base_dev)
+        import torch
+        d_aux = torch.from_numpy(self.helper_columns().view(np.int64)).to(base_dev.device)
+        return _device_extension(len(self.rows), d_aux, [tuple(c) for c in challenges], ctx, base_dev)
 
     def _extension(self, ch):
         """gen_*_ext_matrix (trace.rs:108-279): running products / evaluations, row by row"""
@@ -285,21 +293,122 @@ class BrainfuckTrace(Trace):
         return out
 
 
+# ---------------------------------------------------------------- the trace built on the device (include/ministark_bf.h)
+_CONTEXTS = {}
+
+
+def _torch_device(device):
+    import torch
+    dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+    if dev.type == "cuda" and dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    return dev
+
+
+def _context(dev):
+    """one context per device for building traces, queued on torch's current stream when that is a stream of its own (a
+    handle of 0, the legacy default stream, leaves the context on its own non-blocking stream: callers sync it)"""
+    import torch
+    from .. import Context
+    key = (dev.type, dev.index)
+    if key not in _CONTEXTS:
+        _CONTEXTS[key] = Context(dev.index or 0)
+    ctx = _CONTEXTS[key]
+    if dev.type == "cuda":
+        ctx.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+    return ctx
+
+
+def _device_tables(program, log, dev):
+    """the (17, n) base matrix on `dev` from the program (uint32 words) and the run's records: the table lengths first
+    (one device-to-host sync), then the fill.  The uploaded log and the workspace are freed before it returns, and the
+    matrix is complete: a prover may read it on another stream."""
+    import torch
+    ctx = _context(dev)
+    d_prog = torch.from_numpy(program.view(np.int32)).to(dev)
+    d_log = torch.from_numpy(log.view(np.int64)).to(dev)
+    sizes = ctx.bf_trace_sizes(d_prog, program.size, d_log, log.size)
+    base = torch.empty((17, sizes["n"]), dtype=torch.int64, device=dev)
+    work = torch.empty(sizes["work_bytes"], dtype=torch.uint8, device=dev)
+    if base.is_cuda:                    # the context's stream may not be torch's: torch's own work on this memory is done
+        torch.cuda.current_stream(dev).synchronize()
+    ctx.bf_trace_fill(d_prog, program.size, d_log, log.size, sizes, work, base)
+    ctx.sync()                          # the fill is done before its inputs go back to the allocator and base is handed over
+    del work, d_log, d_prog
+    return base, sizes
+
+
+def _simulate_device(source, input_bytes, device, max_cycles):
+    from .. import bf_run
+    program = np.array(compile_program(source), dtype=np.uint32)
+    log, output = bf_run(program, input_bytes, max_cycles)
+    return BrainfuckDeviceTrace(program, log, _torch_device(device)), output
+
+
+class BrainfuckDeviceTrace(Trace):
+    """The trace of one run with its base columns resident on a device, built from the run's records (ms_bf_run) by
+    ms_bf_trace_sizes / ms_bf_trace_fill; equal word for word to `BrainfuckTrace(rows).base_columns()`.
+
+    The host keeps only the program and the records (8 bytes per processor row).  A prover that no longer needs the
+    natural-order matrix (GpuProver, once the extension columns are built) calls release_base_columns(), so that the
+    proof's peak device memory is what it is for a host trace; base_columns() rebuilds the matrix from the records when
+    asked again."""
+
+    def __init__(self, program, log, device):
+        self.program, self.log, self.device = program, log, device
+        base, self.sizes = _device_tables(program, log, device)
+        super().__init__(base)
+        self.n = self.sizes["n"]
+
+    def __len__(self):
+        return self.n
+
+    def base_columns(self):
+        if self._base is None:
+            self._base, _ = _device_tables(self.program, self.log, self.device)
+        return self._base
+
+    def helper_columns_device(self, ctx, base_dev=None):
+        """BrainfuckTrace.helper_columns() computed on the device from the base matrix: an (8, n) int64 tensor, written on
+        ctx's stream (not synchronised)"""
+        import torch
+        base = self.base_columns() if base_dev is None else base_dev
+        aux = torch.empty((8, self.n), dtype=torch.int64, device=base.device)
+        ctx.bf_helper_columns(base, self.n, aux)
+        return aux
+
+    def release_base_columns(self):
+        """drop the trace's reference to the base matrix (other references keep it alive until they go)"""
+        self._base = None
+
+    def build_extension_columns_device(self, challenges, ctx, base_dev):
+        return _device_extension(self.n, self.helper_columns_device(ctx, base_dev), [tuple(c) for c in challenges], ctx,
+                                 base_dev)
+
+    def to_host(self):
+        """the same trace as a host BrainfuckTrace (downloads the base matrix and decodes it; slow at large n)"""
+        words = self.base_columns().cpu().numpy().view(np.uint64)
+        rows = (words // np.uint64(0xFFFFFFFF)).T.tolist()          # every value but MemValInv is below 2^32
+        for r in rows:
+            r[MEM_VAL_INV] = pow(r[MEM_VAL], -1, P) if r[MEM_VAL] else 0
+        return BrainfuckTrace(rows)
+
+    def build_extension_columns(self, challenges):
+        return self.to_host()._extension(challenges)
+
+
 _FACTOR_PROGRAMS = {}
 
 
-def _device_extension(trace, ch, ctx, base_dev):
+def _device_extension(n, d_aux, ch, ctx, base_dev):
     """The nine extension columns of `BrainfuckTrace._extension`, built on the device: every column is
     x_0 = init, x_(i+1) = x_i * a_i + b_i  with per-row multipliers / addends that are pointwise expressions of the
     base row (evaluated by the fused evaluator over the resident trace) — then one parallel scan (ms_scan_affine).
-    Row conditions that look at neighbouring rows or at opcodes are 0/1 helper columns computed from the integer
-    rows on the host (vectorised numpy, a few bytes per row)."""
+    Row conditions that look at neighbouring rows or at opcodes are the eight 0/1 helper columns `d_aux` (device, (8, n)):
+    computed from the integer rows on the host for a host trace, by ms_bf_helper_columns for a device trace."""
     import torch
     from .. import FP, FQ3, ONE
-    n = len(trace.rows)
     log_n = n.bit_length() - 1
-    aux = trace.helper_columns()
-    d_aux = torch.from_numpy(aux.view(np.int64)).to(base_dev.device)
     NB = 17
     AUX = lambda k: E.Trace(NB + k, 0)
     T, CH = (lambda c: E.Trace(c, 0)), E.Challenge
@@ -307,7 +416,7 @@ def _device_extension(trace, ch, ctx, base_dev):
     instr_fp = lambda ip, c, nx: CH(CH_ALPHA) - CH(CH_A) * ip - CH(CH_B) * c - CH(CH_C) * nx
     mem_fp = lambda cy, mp, v: CH(CH_BETA) - CH(CH_D) * cy - CH(CH_E) * mp - CH(CH_F) * v
     gated = lambda mask, factor: one + mask * (factor - one)                      # factor where mask = 1, else 1
-    cols = [base_dev[c] for c in range(NB)] + [d_aux[k] for k in range(aux.shape[0])]
+    cols = [base_dev[c] for c in range(NB)] + [d_aux[k] for k in range(d_aux.shape[0])]
     is_q = [False] * len(cols)
     sz = 3 * n
 

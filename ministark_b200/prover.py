@@ -333,6 +333,7 @@ class GpuProver:
             leaves, nodes = self._empty(N, 4), self._empty(N, 4)
             base_root = ctx.merkle_commit(base_lde, FP, N, nbase, leaves=leaves, nodes=nodes)
             base_tree = _Tree(leaves, nodes, N)
+        del host_base                           # held no longer than `base`: see release_base_columns below
         channel.commit_base_trace(base_root)
         lap("base_trace_commitment")
         challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
@@ -444,6 +445,7 @@ class GpuProver:
         if tuple(host_base.shape) != (nbase, n):
             raise ProvingError(f"expected {nbase} base columns of {n} rows")
         base = self._to_device(host_base)
+        del host_base                           # held no longer than `base`: see release_base_columns below
         base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
         ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
         base_nodes, base_root = self._commit_blocks(base_polys, base_blk, FP, nbase, log_n, log_b, offsets)
@@ -548,6 +550,9 @@ class GpuProver:
             ext = r.trace.build_extension_columns_device(challenges, r.ctx, base)
         else:
             ext = r.trace.build_extension_columns(challenges)
+        release = getattr(r.trace, "release_base_columns", None)
+        if release is not None:     # the natural-order base matrix is not read from the trace again in this proof
+            release()
         num_ext = 0 if ext is None else int(ext.shape[0])
         if num_ext != r.next_:
             raise ProvingError(f"expected {r.next_} extension columns, got {num_ext}")
