@@ -699,6 +699,11 @@ public:
         int log_ce = (int)log_n + (63 - __builtin_clzll(ce_blowup_factor));
         return compile_program(g, composition.id, num_base_cols, ce_blowup_factor, log_ce, /*batch_inverses=*/true);   // zerofier denominators
     }
+    // the same constraints over one coset block of n rows (ministark_b200/cosets.py::block_program): inside a block the
+    // ce-domain stride is 1 and the domain has n points
+    Program block_program(u32 num_base_cols) {
+        return compile_program(g, composition.id, num_base_cols, 1, (int)log_n, /*batch_inverses=*/true);
+    }
 };
 
 // examples/fib (examples/fib/main.rs:78-150): 8 boundary + 1 terminal + 8 transition constraints

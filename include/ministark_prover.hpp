@@ -3,23 +3,52 @@
 // (prover.rs:56-72) through a device-side column builder; bf::device_extension below builds the nine brainfuck
 // extension columns from the resident base trace with the fused evaluator + ms_scan_affine.
 //
+// Two residencies, chosen per proof as GpuProver (prover.py) chooses them: resident keeps every LDE matrix and tree in
+// device memory; streamed keeps the coefficients and the tree node heaps and recomputes one coset block of the LDE at a
+// time (commitment, constraint evaluation, DEEP), answering queries from the coefficients.  Both emit the same bytes.
+//
 // Host logic (coin, AIR, programs, wire format) comes from ministark_host.hpp and is CPU-tested.  This file only strings
-// the ms_* calls together; it is compile- and link-checked in the build container and exercised on a GPU by
-// tests/test_gpu_cpp_prover.py, which compares its proof bytes with the Python driver's.
+// the ms_* calls together; linked against the CPU build of the ABI it is byte-compared with the CPU restatement of the
+// reference prover, and on a GPU with the Python driver (tests/test_zz_gpu_cpp_prover.py,
+// tests/test_gpu_cpp_stream_prover.py).
 #pragma once
+#include <cstdio>
+#include <memory>
 #include <stdexcept>
 
 #include "ministark_b200.h"
+#include "ministark_bf.h"
+#include "ministark_device.h"
 #include "ministark_examples.hpp"
 #include "ministark_host.hpp"
+#include "ministark_stream.h"
+
+// ministark_b200.h is the ABI every library build exports.  The entry points of the headers beside it are referenced
+// weakly, so that this layer also links against a build that exports the core alone: without ms_device_memory only
+// GpuProver::memory_budget limits a proof, and the streamed residency and the device-built brainfuck trace throw when the
+// library lacks their entry points.
+#pragma weak ms_device_memory
+#pragma weak ms_merkle_commit_block_sha256
+#pragma weak ms_lde_rows
+#pragma weak ms_bf_run
+#pragma weak ms_bf_trace_sizes
+#pragma weak ms_bf_trace_fill
+#pragma weak ms_bf_helper_columns
 
 namespace mshost {
+
+// number of ms_alloc_device calls made through DeviceBuf by this process
+inline u64 &device_allocations() {
+    static u64 count = 0;
+    return count;
+}
 
 struct DeviceBuf {   // RAII over ms_alloc_device
     ms_ctx *ctx = nullptr;
     void *p = nullptr;
     DeviceBuf() = default;
     DeviceBuf(ms_ctx *c, size_t bytes) : ctx(c) {
+        device_allocations()++;
         if (ms_alloc_device(c, bytes, &p) != MS_OK) throw std::runtime_error(std::string("ms_alloc_device: ") + ms_last_error(c));
     }
     DeviceBuf(const DeviceBuf &) = delete;
@@ -83,10 +112,88 @@ inline Expr deep_expression(Graph &g, const std::vector<std::pair<u64, int64_t>>
     return total * (H(DK_DALPHA, 0) + x * H(DK_DBETA, 0));
 }
 
+// ------------------------------------------------------------------------------------------------ residency
+// Device memory the estimates leave free: NTT plans with their twiddle and scale tables, the NTT temporary and the
+// context's scratch arenas (prover.py MEMORY_RESERVE).
+constexpr u64 MEMORY_RESERVE = (u64)3 << 30;
+
+struct PeakBytes { u64 resident, streamed; };
+
+// Peak device bytes of one proof in each residency, from the shapes (prover.py peak_bytes).  lanes: 1 for Fq = Fp, 3 for
+// Fq3; ce_blowup: the composition blow-up; ff: the FRI folding factor.
+inline PeakBytes peak_bytes(u64 n, u64 beta, u64 nbase, u64 next, u64 lanes, u64 ce_blowup, u64 ff = 2) {
+    const u64 N = n * beta, M = n * ce_blowup;
+    const u64 words = nbase + lanes * (next + ce_blowup);
+    const u64 ntrees = next ? 3 : 2;
+    const u64 fri = (8 * lanes + 64) * N / (ff - 1);
+    const u64 common = 8 * words * n + 8 * N * lanes + fri + ((u64)16 << 20);
+    return {common + 8 * M * lanes + 8 * words * N + 64 * ntrees * N, common + 8 * words * n + 32 * ntrees * N + 32 * n};
+}
+
+inline std::string gib(long double b) {
+    char s[64];
+    snprintf(s, sizeof s, "%.2Lf GiB", b / (long double)((u64)1 << 30));
+    return s;
+}
+
+// ------------------------------------------------------------------------------------------------ coset blocks
+// ministark_b200/cosets.py: block q of the bit-reversed LDE over 7 * <g_N> is the size-n transform over the coset
+// h_q * <g_n>, h_q = 7 * g_N^bitrev(q).  Returns the Montgomery words of h_0 .. h_(2^log_b - 1).
+inline u64 bit_reverse_bits(u64 v, unsigned bits) {
+    u64 r = 0;
+    for (unsigned i = 0; i < bits; i++, v >>= 1) r = (r << 1) | (v & 1);
+    return r;
+}
+inline std::vector<u64> coset_offsets(unsigned log_n, unsigned log_b) {
+    const u64 gN = domain_generator(log_n + log_b);
+    std::vector<u64> h;
+    for (u64 q = 0; q < ((u64)1 << log_b); q++) h.push_back(to_mont(mulm(GENERATOR, powm(gN, bit_reverse_bits(q, log_b)))));
+    return h;
+}
+
+// The index walk of MerkleTreeImpl::prove (src/merkle.rs:149-207): which leaves and which heap nodes a batched proof of
+// `indices` names (cosets.py merkle_walk).
+struct MerkleWalk { std::vector<u64> init, sib, path; };
+inline MerkleWalk merkle_walk(u64 n_leaves, const std::vector<u64> &indices) {
+    const std::set<u64> s(indices.begin(), indices.end());
+    const std::vector<u64> idx(s.begin(), s.end());
+    MerkleWalk w;
+    std::vector<u64> node_q;
+    for (size_t k = 0; k < idx.size();) {
+        const u64 i = idx[k];
+        w.init.push_back(i);
+        node_q.push_back((n_leaves + i) >> 1);
+        if (k + 1 < idx.size() && (i ^ 1) == idx[k + 1]) {
+            w.init.push_back(idx[k + 1]);
+            k += 2;
+            continue;
+        }
+        w.sib.push_back(i ^ 1);
+        k++;
+    }
+    for (size_t head = 0; head < node_q.size();) {
+        const u64 i = node_q[head++];
+        if (i > 2) node_q.push_back(i >> 1);
+        if (head < node_q.size() && (i ^ 1) == node_q[head]) {
+            head++;
+            continue;
+        }
+        w.path.push_back(i ^ 1);
+    }
+    return w;
+}
+
 class GpuProver {
     ms_ctx *ctx = nullptr;
 
 public:
+    // bytes one proof may use on the device; 0: whatever the device has free
+    u64 memory_budget = 0;
+    // "resident" or "streamed": what the last proof ran (empty before the first)
+    std::string last_residency;
+    // the lowest free device memory ms_device_memory reported between the phases of the last proof
+    u64 lowest_free_bytes = 0;
+
     explicit GpuProver(int device = 0) {
         if (ms_ctx_create(device, &ctx) != MS_OK) throw std::runtime_error("ms_ctx_create failed (no CUDA device? there is no CPU fallback)");
     }
@@ -99,49 +206,139 @@ public:
     using ExtensionBuilder = std::function<DeviceBuf(ms_ctx *, const u64 *base_dev, u64 n, const std::vector<Fq> &challenges)>;
     ms_ctx *context() const { return ctx; }
 
+    // free device memory as the driver reports it (SIZE_MAX where the library has no device limit or no ms_device_memory)
+    u64 free_memory() const {
+        if (!ms_device_memory) return SIZE_MAX;
+        size_t f = 0;
+        ck(ctx, ms_device_memory(ctx, &f, nullptr), "ms_device_memory");
+        return f;
+    }
+    // bytes a proof may allocate: free device memory minus MEMORY_RESERVE, capped by memory_budget (prover.py
+    // memory_available; there is no allocator cache to add back).  Negative when the device is nearly full.
+    int64_t memory_available() const {
+        const u64 f = free_memory();
+        const int64_t avail = (f >= (u64)INT64_MAX ? INT64_MAX : (int64_t)f) - (int64_t)MEMORY_RESERVE;
+        return memory_budget ? std::min<int64_t>((int64_t)memory_budget, avail) : avail;
+    }
+    // "resident" if its estimate fits, else "streamed" if that fits, else the refusal (nothing is allocated yet)
+    std::string choose_residency(const PeakBytes &est) const {
+        const int64_t budget = memory_available();
+        if ((int64_t)est.resident <= budget) return "resident";
+        if ((int64_t)est.streamed <= budget) return "streamed";
+        throw std::runtime_error("the proof does not fit on the device: it needs about " + gib(est.resident) + " resident or " +
+                                 gib(est.streamed) + " streamed, and " + gib(budget) + " is available");
+    }
+
     // base_trace: num_base_columns x n Montgomery words, column-major, HOST memory.  public_inputs: handed to gen_hints;
     // public_inputs_bytes: their CanonicalSerialize form for the coin seed (empty: the Fq elements back to back, as for
-    // examples/fib's single claimed value).
+    // examples/fib's single claimed value).  The trace is not read when the proof does not fit (std::runtime_error).
     Proof prove(const AirConfig &cfg, ProofOptions options, const u64 *base_trace, u64 n, const std::vector<Fq> &public_inputs,
                 const Bytes &public_inputs_bytes = {}, const ExtensionBuilder &ext_builder = nullptr) {
+        DeviceBuf none;
+        return prove_any(cfg, options, base_trace, none, n, public_inputs, public_inputs_bytes, ext_builder);
+    }
+    // the same from a DEVICE trace (num_base_columns x n, column-major, allocated on this prover's context), whose
+    // ownership passes to the prover: it is freed as soon as the extension columns are built (ministark_b200's
+    // release_base_columns), so the proof's peak device memory is the host trace's.
+    Proof prove(const AirConfig &cfg, ProofOptions options, DeviceBuf base_trace, u64 n, const std::vector<Fq> &public_inputs,
+                const Bytes &public_inputs_bytes = {}, const ExtensionBuilder &ext_builder = nullptr) {
+        if (!base_trace.p || base_trace.ctx != ctx) throw std::runtime_error("the device trace must be allocated on this prover's context");
+        return prove_any(cfg, options, nullptr, base_trace, n, public_inputs, public_inputs_bytes, ext_builder);
+    }
+
+private:
+    struct Run {                    // per-proof state shared by the phases of both residencies
+        const AirConfig &cfg;
+        ProofOptions options;
+        Air air;
+        const std::vector<Fq> &public_inputs;
+        const ExtensionBuilder &ext_builder;
+        PublicCoin coin;
+        Proof proof;
+        int fq, lanes;
+        unsigned log_n, log_b, log_N, log_ce;
+        u64 n, N, ce, M, GEN, ONE;
+        u32 nbase, next;
+        const u64 *host_trace;      // exactly one of host_trace / device_trace holds the base trace
+        DeviceBuf &device_trace;
+    };
+
+    void note_memory() { lowest_free_bytes = std::min<u64>(lowest_free_bytes, free_memory()); }
+
+    Proof prove_any(const AirConfig &cfg, ProofOptions options, const u64 *host_trace, DeviceBuf &device_trace, u64 n,
+                    const std::vector<Fq> &public_inputs, const Bytes &public_inputs_bytes, const ExtensionBuilder &ext_builder) {
         const u32 next = cfg.num_extension_columns;
         if (next && !ext_builder) throw std::runtime_error("this AIR has extension columns: pass an ExtensionBuilder");
-        const int fq = cfg.fq_is_fp ? MS_FIELD_FP : MS_FIELD_FQ3, lanes = cfg.fq_is_fp ? 1 : 3;
-        Air air(cfg, n, options);
-        const unsigned log_n = air.log_n, beta = options.lde_blowup_factor, log_b = 31 - (unsigned)__builtin_clz(beta);
-        const unsigned log_N = log_n + log_b;
-        const u64 N = n << log_b, ce = air.ce_blowup_factor, M = n * ce;
-        const unsigned log_ce = log_n + (63 - (unsigned)__builtin_clzll(ce));
-        const u32 nbase = cfg.num_base_columns;
-        const u64 GEN = to_mont(GENERATOR), ONE = to_mont(1);
+        const int lanes = cfg.fq_is_fp ? 1 : 3;
         // gen_public_coin (examples/fib/main.rs:166-172)
         Bytes seed = public_inputs_bytes;
         if (seed.empty())
             for (const Fq &v : public_inputs) put_elem(seed, v, lanes);
         put_u64_le(seed, n);
         for (u8 b : options.to_bytes()) seed.push_back(b);
-        PublicCoin coin(sha256({seed}), lanes);
-        Proof proof;
-        proof.options = options;
-        proof.trace_len = n;
+        Run r{cfg, options, Air(cfg, n, options), public_inputs, ext_builder, PublicCoin(sha256({seed}), lanes), Proof{},
+              cfg.fq_is_fp ? MS_FIELD_FP : MS_FIELD_FQ3, lanes, 0, 0, 0, 0, n, 0, 0, 0, to_mont(GENERATOR), to_mont(1),
+              cfg.num_base_columns, next, host_trace, device_trace};
+        const unsigned beta = options.lde_blowup_factor;
+        r.log_n = r.air.log_n;
+        r.log_b = 31 - (unsigned)__builtin_clz(beta);
+        r.log_N = r.log_n + r.log_b;
+        r.N = n << r.log_b;
+        r.ce = r.air.ce_blowup_factor;
+        r.M = n * r.ce;
+        r.log_ce = r.log_n + (63 - (unsigned)__builtin_clzll(r.ce));
+        r.proof.options = options;
+        r.proof.trace_len = n;
+        last_residency = choose_residency(peak_bytes(n, beta, r.nbase, next, lanes, r.ce, options.fri_folding_factor));
+        lowest_free_bytes = UINT64_MAX;
+        note_memory();
+        if (last_residency == "resident") prove_resident(r);
+        else prove_streamed(r);
+        note_memory();
+        return std::move(r.proof);
+    }
+
+    // the base trace on the device: the handed-over device matrix, or a fresh upload of the host one
+    DeviceBuf device_base(Run &r) {
+        if (r.device_trace.p) return std::move(r.device_trace);
+        DeviceBuf d(ctx, (size_t)r.nbase * r.n * 8);
+        ck(ctx, ms_copy(ctx, d.p, r.host_trace, (size_t)r.nbase * r.n * 8), "upload");
+        return d;
+    }
+
+    // challenges drawn after the base commitment, then the extension columns built from the natural-order base matrix,
+    // which is freed as soon as they exist
+    DeviceBuf extension_columns(Run &r, DeviceBuf &d_trace, std::vector<Fq> &challenges, std::vector<Fq> &hints) {
+        for (u64 i = 0; i < r.air.num_challenges(); i++) challenges.push_back(r.coin.draw());
+        hints = r.cfg.gen_hints ? r.cfg.gen_hints(r.n, r.public_inputs, challenges) : std::vector<Fq>{};
+        DeviceBuf ext;
+        if (r.next) ext = r.ext_builder(ctx, d_trace.words(), r.n, challenges);
+        d_trace.release();
+        return ext;
+    }
+
+    void prove_resident(Run &r) {
+        const u64 n = r.n, N = r.N, ce = r.ce, M = r.M, GEN = r.GEN, ONE = r.ONE;
+        const unsigned log_n = r.log_n, log_b = r.log_b, log_N = r.log_N, log_ce = r.log_ce;
+        const u32 nbase = r.nbase, next = r.next;
+        const int fq = r.fq, lanes = r.lanes;
+        Proof &proof = r.proof;
 
         // ---- base trace commitment (prover.rs:46-55)
-        DeviceBuf d_trace(ctx, (size_t)nbase * n * 8), base_polys(ctx, (size_t)nbase * n * 8), base_lde(ctx, (size_t)nbase * N * 8);
+        DeviceBuf d_trace = device_base(r), base_polys(ctx, (size_t)nbase * n * 8), base_lde(ctx, (size_t)nbase * N * 8);
         DeviceBuf base_leaves(ctx, N * 32), base_nodes(ctx, N * 32);
-        ck(ctx, ms_copy(ctx, d_trace.p, base_trace, (size_t)nbase * n * 8), "upload");
         ck(ctx, ms_ntt_batch_to(ctx, MS_FIELD_FP, d_trace.p, n, base_polys.p, n, nbase, log_n, MS_NTT_INVERSE, ONE), "interpolate");
         ck(ctx, ms_lde_batch(ctx, MS_FIELD_FP, base_polys.p, n, base_lde.p, N, nbase, log_n, log_b, GEN, 1), "lde");
         proof.base_trace_commitment.resize(32);
         ck(ctx, ms_merkle_commit_sha256(ctx, MS_FIELD_FP, base_lde.p, N, nbase, N, base_leaves.p, base_nodes.p, proof.base_trace_commitment.data()), "commit");
-        coin.reseed_with_digest(proof.base_trace_commitment);
-        std::vector<Fq> challenges;
-        for (u64 i = 0; i < air.num_challenges(); i++) challenges.push_back(coin.draw());
-        const std::vector<Fq> hints = cfg.gen_hints ? cfg.gen_hints(n, public_inputs, challenges) : std::vector<Fq>{};
+        r.coin.reseed_with_digest(proof.base_trace_commitment);
+        note_memory();
 
         // ---- extension trace commitment (prover.rs:56-72)
+        std::vector<Fq> challenges, hints;
+        DeviceBuf ext = extension_columns(r, d_trace, challenges, hints);
         DeviceBuf ext_polys, ext_lde, ext_leaves, ext_nodes;
         if (next) {
-            DeviceBuf ext = ext_builder(ctx, d_trace.words(), n, challenges);
             ext_polys = DeviceBuf(ctx, (size_t)next * n * lanes * 8);
             ext_lde = DeviceBuf(ctx, (size_t)next * N * lanes * 8);
             ext_leaves = DeviceBuf(ctx, N * 32);
@@ -152,17 +349,19 @@ public:
             proof.extension_trace_commitment.resize(32);
             ck(ctx, ms_merkle_commit_sha256(ctx, fq, ext_lde.p, N, next, N, ext_leaves.p, ext_nodes.p, proof.extension_trace_commitment.data()),
                "extension commit");
-            coin.reseed_with_digest(proof.extension_trace_commitment);
+            r.coin.reseed_with_digest(proof.extension_trace_commitment);
         }
-        d_trace.release();
+        ext.release();
+        note_memory();
 
         // ---- constraint evaluation over the ce domain, read in place from the bit-reversed LDE prefix (prover.rs:75-108)
         std::vector<Fq> ccoefs;
-        for (u64 i = 0; i < air.num_composition_constraint_coeffs(); i++) ccoefs.push_back(coin.draw());
-        const Program prog = air.composition_program(nbase).bind(challenges, hints, ccoefs);
+        for (u64 i = 0; i < r.air.num_composition_constraint_coeffs(); i++) ccoefs.push_back(r.coin.draw());
+        const Program prog = r.air.composition_program(nbase).bind(challenges, hints, ccoefs);
         DeviceBuf comp_evals(ctx, M * lanes * 8);
         ck(ctx, ms_eval_constraints(ctx, &prog.code[0][0], (unsigned)prog.code.size(), &prog.consts[0][0], (unsigned)prog.consts.size(),
                                     base_lde.p, N, nbase, next ? ext_lde.p : nullptr, N, next, fq, log_ce, GEN, 1, 0, comp_evals.p), "eval_constraints");
+        note_memory();
 
         // ---- composition trace (prover.rs:110-125)
         ck(ctx, ms_ntt_batch(ctx, fq, comp_evals.p, M, 1, log_ce, MS_NTT_INVERSE, GEN), "composition iNTT");
@@ -178,16 +377,240 @@ public:
         proof.composition_trace_commitment.resize(32);
         ck(ctx, ms_merkle_commit_sha256(ctx, fq, comp_lde.p, N, (unsigned)ce, N, comp_leaves.p, comp_nodes.p, proof.composition_trace_commitment.data()),
            "composition commit");
-        coin.reseed_with_digest(proof.composition_trace_commitment);
+        r.coin.reseed_with_digest(proof.composition_trace_commitment);
+        note_memory();
 
-        // ---- out-of-domain evaluations (composer.rs:43-86)
-        const Fq z = coin.draw();
-        const auto trace_args = air.trace_arguments();
+        // ---- DEEP composition evaluated over the LDE domain (composer.rs:89-188 in evaluation form)
+        const Program dprog = bind_deep(r, base_polys.p, ext_polys.p, comp_polys);
+        std::vector<const void *> cols;
+        std::vector<int> is_q;
+        for (u32 c = 0; c < nbase; c++) { cols.push_back(base_lde.words() + (size_t)c * N); is_q.push_back(0); }
+        for (u32 c = 0; c < next; c++) { cols.push_back(ext_lde.words() + (size_t)c * N * lanes); is_q.push_back(1); }
+        for (u64 j = 0; j < ce; j++) { cols.push_back(comp_lde.words() + (size_t)j * N * lanes); is_q.push_back(1); }
+        DeviceBuf cur(ctx, N * lanes * 8);
+        ck(ctx, ms_eval_constraints_ptrs(ctx, &dprog.code[0][0], (unsigned)dprog.code.size(), &dprog.consts[0][0], (unsigned)dprog.consts.size(),
+                                         cols.data(), is_q.data(), (unsigned)cols.size(), fq, log_N, GEN, 1, 1, cur.p), "deep composition");
+        note_memory();
+
+        // ---- FRI, proof of work, FRI queries; then the trace rows and their paths from the resident trees
+        const std::vector<u64> positions = fri_and_queries(r, cur);
+        std::vector<u64> brow(positions.size() * nbase), crow(positions.size() * ce * lanes);
+        ck(ctx, ms_gather_rows(ctx, MS_FIELD_FP, base_lde.p, N, nbase, N, positions.data(), (unsigned)positions.size(), brow.data()), "base rows");
+        ck(ctx, ms_gather_rows(ctx, fq, comp_lde.p, N, (unsigned)ce, N, positions.data(), (unsigned)positions.size(), crow.data()), "composition rows");
+        proof.trace_queries.base_trace_values = canon_vec(brow, 1);
+        proof.trace_queries.composition_trace_values = canon_vec(crow, lanes);
+        if (next) {
+            std::vector<u64> erow(positions.size() * next * lanes);
+            ck(ctx, ms_gather_rows(ctx, fq, ext_lde.p, N, next, N, positions.data(), (unsigned)positions.size(), erow.data()), "extension rows");
+            proof.trace_queries.extension_trace_values = canon_vec(erow, lanes);
+            proof.trace_queries.has_extension = true;
+            proof.trace_queries.extension_trace_proof = view_of(ext_leaves, ext_nodes, N, positions);
+        }
+        proof.trace_queries.base_trace_proof = view_of(base_leaves, base_nodes, N, positions);
+        proof.trace_queries.composition_trace_proof = view_of(comp_leaves, comp_nodes, N, positions);
+    }
+
+    // ---- streamed residency: coefficients and tree nodes stay, coset blocks are recomputed
+    // coset block with offset h of the bit-reversed LDE of every column of `polys`, into `blk`.  Its NTT plan is dropped at
+    // once: every block has its own offset, and beta cached plans with their full tables would take back the memory
+    // streaming saves.
+    void lde_block(const void *polys, void *blk, int field, unsigned ncols, unsigned log_n, u64 h) {
+        const u64 n = (u64)1 << log_n;
+        ck(ctx, ms_lde_batch(ctx, field, polys, n, blk, n, ncols, log_n, 0, h, 1), "block lde");
+        ck(ctx, ms_set_option(ctx, "drop_plans", 1), "drop_plans");
+    }
+
+    // Merkle commitment of the bit-reversed LDE of `polys`, one coset block at a time: block q is transformed into `blk`
+    // and hashed into its subtree of the node heap; the top log_b levels come from the block roots.  Returns the node heap
+    // and writes the root.
+    DeviceBuf commit_blocks(Run &r, const void *polys, void *blk, int field, unsigned ncols, const std::vector<u64> &offsets, Bytes &root) {
+        const u64 beta = (u64)1 << r.log_b;
+        DeviceBuf nodes(ctx, r.N * 32), roots(ctx, beta * 32);
+        for (u64 q = 0; q < beta; q++) {
+            lde_block(polys, blk, field, ncols, r.log_n, offsets[q]);
+            ck(ctx, ms_merkle_commit_block_sha256(ctx, field, blk, r.n, ncols, r.log_n, r.log_b, q, nodes.p, static_cast<u8 *>(roots.p) + 32 * q),
+               "block commit");
+        }
+        if (beta > 1) ck(ctx, ms_merkle_nodes_sha256(ctx, roots.p, beta, nodes.p), "block roots");
+        const u8 zero[32] = {0};          // the unused default digest (named by a walk over a 2-leaf tree)
+        ck(ctx, ms_copy(ctx, nodes.p, zero, 32), "node 0");
+        root.resize(32);
+        ck(ctx, ms_copy(ctx, root.data(), static_cast<u8 *>(nodes.p) + 32, 32), "root");
+        return nodes;
+    }
+
+    // the rows at `positions` and their MerkleView without the LDE: rows and leaf digests from the coefficients
+    // (ms_lde_rows), path nodes gathered from the resident node heap
+    MerkleView streamed_rows(Run &r, const void *polys, int field, unsigned ncols, const DeviceBuf &nodes, const std::vector<u64> &positions,
+                             std::vector<u64> &rows) {
+        const MerkleWalk w = merkle_walk(r.N, positions);
+        std::vector<u64> ids = positions;
+        ids.insert(ids.end(), w.init.begin(), w.init.end());
+        ids.insert(ids.end(), w.sib.begin(), w.sib.end());
+        const size_t row_words = (size_t)ncols * field;
+        std::vector<u64> all(ids.size() * row_words);
+        ck(ctx, ms_lde_rows(ctx, field, polys, r.n, ncols, r.log_n, r.log_b, r.GEN, ids.data(), (unsigned)ids.size(), all.data()), "lde rows");
+        rows.assign(all.begin(), all.begin() + positions.size() * row_words);
+        MerkleView v;
+        for (size_t k = positions.size(); k < ids.size(); k++) {   // hash_rows: canonical words, 8 bytes little-endian each
+            Bytes ser;
+            for (size_t j = 0; j < row_words; j++) put_u64_le(ser, from_mont(all[k * row_words + j]));
+            (k < positions.size() + w.init.size() ? v.initial_leaves : v.sibling_leaves).push_back(sha256({ser}));
+        }
+        if (!w.path.empty()) {
+            std::vector<u8> path(w.path.size() * 32);
+            ck(ctx, ms_gather_rows_rowmajor(ctx, nodes.p, 4, r.N, w.path.data(), (unsigned)w.path.size(), path.data()), "path nodes");
+            for (size_t i = 0; i < w.path.size(); i++) v.nodes.emplace_back(path.begin() + 32 * i, path.begin() + 32 * i + 32);
+        }
+        v.height = r.log_N;
+        return v;
+    }
+
+    void prove_streamed(Run &r) {
+        const u64 n = r.n, N = r.N, ce = r.ce, M = r.M, GEN = r.GEN, ONE = r.ONE;
+        const unsigned log_n = r.log_n, log_ce = r.log_ce;
+        const u32 nbase = r.nbase, next = r.next;
+        const int fq = r.fq, lanes = r.lanes;
+        Proof &proof = r.proof;
+        if (!ms_merkle_commit_block_sha256 || !ms_lde_rows) throw std::runtime_error("the library lacks the streamed residency (ministark_stream.h)");
+        const std::vector<u64> offsets = coset_offsets(log_n, r.log_b);
+
+        // ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
+        DeviceBuf d_trace = device_base(r), base_polys(ctx, (size_t)nbase * n * 8), base_blk(ctx, (size_t)nbase * n * 8);
+        ck(ctx, ms_ntt_batch_to(ctx, MS_FIELD_FP, d_trace.p, n, base_polys.p, n, nbase, log_n, MS_NTT_INVERSE, ONE), "interpolate");
+        DeviceBuf base_nodes = commit_blocks(r, base_polys.p, base_blk.p, MS_FIELD_FP, nbase, offsets, proof.base_trace_commitment);
+        r.coin.reseed_with_digest(proof.base_trace_commitment);
+        note_memory();
+
+        // ---- extension trace commitment
+        std::vector<Fq> challenges, hints;
+        DeviceBuf ext = extension_columns(r, d_trace, challenges, hints);
+        DeviceBuf ext_polys, ext_blk, ext_nodes;
+        if (next) {
+            ext_polys = DeviceBuf(ctx, (size_t)next * n * lanes * 8);
+            ck(ctx, ms_ntt_batch_to(ctx, fq, ext.p, n, ext_polys.p, n, next, log_n, MS_NTT_INVERSE, ONE), "extension interpolate");
+            ext.release();
+            ext_blk = DeviceBuf(ctx, (size_t)next * n * lanes * 8);
+            ext_nodes = commit_blocks(r, ext_polys.p, ext_blk.p, fq, next, offsets, proof.extension_trace_commitment);
+            proof.has_extension = true;
+            r.coin.reseed_with_digest(proof.extension_trace_commitment);
+        }
+        note_memory();
+
+        auto trace_block = [&](u64 h) {
+            lde_block(base_polys.p, base_blk.p, MS_FIELD_FP, nbase, log_n, h);
+            std::vector<const void *> cols;
+            for (u32 c = 0; c < nbase; c++) cols.push_back(base_blk.words() + (size_t)c * n);
+            if (next) {
+                lde_block(ext_polys.p, ext_blk.p, fq, next, log_n, h);
+                for (u32 c = 0; c < next; c++) cols.push_back(ext_blk.words() + (size_t)c * n * lanes);
+            }
+            return cols;
+        };
+
+        // ---- constraint evaluation, block by block: the blocks q < ce_blowup of the LDE are the ce domain
+        std::vector<Fq> ccoefs;
+        for (u64 i = 0; i < r.air.num_composition_constraint_coeffs(); i++) ccoefs.push_back(r.coin.draw());
+        const Program prog = r.air.block_program(nbase).bind(challenges, hints, ccoefs);
+        DeviceBuf comp_evals(ctx, M * lanes * 8);
+        std::vector<int> is_q(nbase, 0);
+        is_q.resize(nbase + next, 1);
+        for (u64 q = 0; q < ce; q++) {
+            const std::vector<const void *> cols = trace_block(offsets[q]);
+            ck(ctx, ms_eval_constraints_ptrs(ctx, &prog.code[0][0], (unsigned)prog.code.size(), &prog.consts[0][0], (unsigned)prog.consts.size(),
+                                             cols.data(), is_q.data(), (unsigned)cols.size(), fq, log_n, offsets[q], 1, 1,
+                                             comp_evals.words() + q * n * lanes), "eval_constraints (block)");
+        }
+        note_memory();
+
+        // ---- composition trace: the bit-reversed ce-domain column -> coefficients -> ce_blowup columns
+        ck(ctx, ms_bit_reverse(ctx, fq, comp_evals.p, M, 1, log_ce), "composition bit reverse");
+        ck(ctx, ms_ntt_batch(ctx, fq, comp_evals.p, M, 1, log_ce, MS_NTT_INVERSE, GEN), "composition iNTT");
+        DeviceBuf comp_split;
+        if (ce > 1) {
+            comp_split = DeviceBuf(ctx, M * lanes * 8);
+            ck(ctx, ms_matrix_from_rows(ctx, fq, comp_evals.p, n, (unsigned)ce, comp_split.p, n), "composition split");
+            comp_evals.release();
+        }
+        const void *comp_polys = ce > 1 ? comp_split.p : comp_evals.p;
+        ck(ctx, ms_set_option(ctx, "drop_scratch", 1), "drop_scratch");   // the size-M transform's temporary
+        DeviceBuf comp_blk(ctx, ce * n * lanes * 8);
+        DeviceBuf comp_nodes = commit_blocks(r, comp_polys, comp_blk.p, fq, (unsigned)ce, offsets, proof.composition_trace_commitment);
+        r.coin.reseed_with_digest(proof.composition_trace_commitment);
+        note_memory();
+
+        // ---- DEEP composition polynomial: every block of the three matrices recomputed once more
+        const Program dprog = bind_deep(r, base_polys.p, ext_polys.p, comp_polys);
+        DeviceBuf deep(ctx, N * lanes * 8);
+        is_q.resize(nbase + next + ce, 1);
+        for (u64 q = 0; q < offsets.size(); q++) {
+            std::vector<const void *> cols = trace_block(offsets[q]);
+            lde_block(comp_polys, comp_blk.p, fq, (unsigned)ce, log_n, offsets[q]);
+            for (u64 j = 0; j < ce; j++) cols.push_back(comp_blk.words() + j * n * lanes);
+            ck(ctx, ms_eval_constraints_ptrs(ctx, &dprog.code[0][0], (unsigned)dprog.code.size(), &dprog.consts[0][0], (unsigned)dprog.consts.size(),
+                                             cols.data(), is_q.data(), (unsigned)cols.size(), fq, log_n, offsets[q], 1, 1,
+                                             deep.words() + q * n * lanes), "deep composition (block)");
+        }
+        note_memory();                  // the high point: the codeword and one block of every matrix besides the rest
+        base_blk.release();
+        ext_blk.release();
+        comp_blk.release();
+
+        // ---- FRI, proof of work, FRI queries; then rows and leaf digests from the coefficients, paths from the node heaps
+        const std::vector<u64> positions = fri_and_queries(r, deep);
+        std::vector<u64> rows;
+        Queries &tq = proof.trace_queries;
+        tq.base_trace_proof = streamed_rows(r, base_polys.p, MS_FIELD_FP, nbase, base_nodes, positions, rows);
+        tq.base_trace_values = canon_vec(rows, 1);
+        tq.composition_trace_proof = streamed_rows(r, comp_polys, fq, (unsigned)ce, comp_nodes, positions, rows);
+        tq.composition_trace_values = canon_vec(rows, lanes);
+        if (next) {
+            tq.extension_trace_proof = streamed_rows(r, ext_polys.p, fq, next, ext_nodes, positions, rows);
+            tq.extension_trace_values = canon_vec(rows, lanes);
+            tq.has_extension = true;
+        }
+    }
+
+    // ---- phases both residencies share
+    static std::vector<Fq> canon_vec(const std::vector<u64> &w, int l) {
+        std::vector<Fq> o;
+        for (size_t i = 0; i < w.size(); i += l) {
+            Fq v;
+            for (int k = 0; k < l; k++) v.c[k] = from_mont(w[i + k]);
+            o.push_back(v);
+        }
+        return o;
+    }
+
+    MerkleView view_of(const DeviceBuf &leaves, const DeviceBuf &nodes, u64 nleaves, const std::vector<u64> &idx) {
+        const unsigned height = 63 - (unsigned)__builtin_clzll(nleaves);
+        std::vector<u8> init(idx.size() * 32), sib(idx.size() * 32), path(idx.size() * (height ? height : 1) * 32);
+        unsigned counts[3];
+        ck(ctx, ms_merkle_prove_sha256(ctx, leaves.p, nodes.p, nleaves, idx.data(), (unsigned)idx.size(), init.data(), sib.data(), path.data(), counts),
+           "merkle prove");
+        MerkleView v;
+        auto take = [](const std::vector<u8> &b, unsigned k) { std::vector<Bytes> o; for (unsigned i = 0; i < k; i++) o.emplace_back(b.begin() + 32 * i, b.begin() + 32 * i + 32); return o; };
+        v.initial_leaves = take(init, counts[0]);
+        v.sibling_leaves = take(sib, counts[1]);
+        v.nodes = take(path, counts[2]);
+        v.height = height;
+        return v;
+    }
+
+    // out-of-domain evaluations (composer.rs:43-86) from the coefficients, into the proof and the coin; then the DEEP
+    // coefficients are drawn and bound into the DEEP program
+    Program bind_deep(Run &r, const void *base_polys, const void *ext_polys, const void *comp_polys) {
+        const u64 n = r.n, ce = r.ce;
+        const u32 nbase = r.nbase, next = r.next;
+        const int fq = r.fq, lanes = r.lanes;
+        Proof &proof = r.proof;
+        const Fq z = r.coin.draw();
+        const auto trace_args = r.air.trace_arguments();
         std::vector<int64_t> offsets;
         for (const auto &ta : trace_args)
             if (std::find(offsets.begin(), offsets.end(), ta.second) == offsets.end()) offsets.push_back(ta.second);
         std::sort(offsets.begin(), offsets.end());
-        const u64 g = domain_generator(log_n), g_inv = invm(g);
+        const u64 g = domain_generator(r.log_n), g_inv = invm(g);
         std::vector<Fq> z_points;
         std::vector<u64> pts;
         for (int64_t o : offsets) {
@@ -197,9 +620,9 @@ public:
         }
         const Fq z_m = fq_pow(z, ce);
         std::vector<u64> base_ood((size_t)nbase * offsets.size() * 3), comp_ood(ce * 3);
-        ck(ctx, ms_poly_eval(ctx, MS_FIELD_FP, base_polys.p, n, nbase, n, pts.data(), (unsigned)offsets.size(), base_ood.data()), "ood (trace)");
+        ck(ctx, ms_poly_eval(ctx, MS_FIELD_FP, base_polys, n, nbase, n, pts.data(), (unsigned)offsets.size(), base_ood.data()), "ood (trace)");
         std::vector<u64> ext_ood((size_t)next * offsets.size() * 3);
-        if (next) ck(ctx, ms_poly_eval(ctx, fq, ext_polys.p, n, next, n, pts.data(), (unsigned)offsets.size(), ext_ood.data()), "ood (extension)");
+        if (next) ck(ctx, ms_poly_eval(ctx, fq, ext_polys, n, next, n, pts.data(), (unsigned)offsets.size(), ext_ood.data()), "ood (extension)");
         const u64 zm_w[3] = {to_mont(z_m.c[0]), to_mont(z_m.c[1]), to_mont(z_m.c[2])};
         ck(ctx, ms_poly_eval(ctx, fq, comp_polys, n, (unsigned)ce, n, zm_w, 1, comp_ood.data()), "ood (composition)");
         auto canon3 = [&](const u64 *w) {
@@ -216,13 +639,12 @@ public:
         for (u64 j = 0; j < ce; j++) proof.composition_trace_ood_evals.push_back(canon3(&comp_ood[j * 3]));
         std::vector<Fq> all_oods = proof.execution_trace_ood_evals;
         all_oods.insert(all_oods.end(), proof.composition_trace_ood_evals.begin(), proof.composition_trace_ood_evals.end());
-        coin.reseed_with_field_elements(all_oods);
+        r.coin.reseed_with_field_elements(all_oods);
 
-        // ---- DEEP composition evaluated over the LDE domain (composer.rs:89-188 in evaluation form)
         std::vector<Fq> ex_alphas, co_alphas;
-        for (size_t i = 0; i < trace_args.size(); i++) ex_alphas.push_back(coin.draw());
-        for (u64 j = 0; j < ce; j++) co_alphas.push_back(coin.draw());
-        const Fq d_alpha = coin.draw(), d_beta = coin.draw();
+        for (size_t i = 0; i < trace_args.size(); i++) ex_alphas.push_back(r.coin.draw());
+        for (u64 j = 0; j < ce; j++) co_alphas.push_back(r.coin.draw());
+        const Fq d_alpha = r.coin.draw(), d_beta = r.coin.draw();
         Graph dg;
         std::vector<DeepKey> keys;
         const Expr dexpr = deep_expression(dg, trace_args, nbase + next, (u32)ce, keys);
@@ -250,22 +672,21 @@ public:
                 default: dhints.push_back(d_beta);
             }
         }
-        const Program dprog = compile_program(dg, dexpr.id, nbase, 1, (int)log_N, /*batch_inverses=*/true).bind({}, dhints, {});
-        std::vector<const void *> cols;
-        std::vector<int> is_q;
-        for (u32 c = 0; c < nbase; c++) { cols.push_back(base_lde.words() + (size_t)c * N); is_q.push_back(0); }
-        for (u32 c = 0; c < next; c++) { cols.push_back(ext_lde.words() + (size_t)c * N * lanes); is_q.push_back(1); }
-        for (u64 j = 0; j < ce; j++) { cols.push_back(comp_lde.words() + (size_t)j * N * lanes); is_q.push_back(1); }
-        DeviceBuf cur(ctx, N * lanes * 8);
-        ck(ctx, ms_eval_constraints_ptrs(ctx, &dprog.code[0][0], (unsigned)dprog.code.size(), &dprog.consts[0][0], (unsigned)dprog.consts.size(),
-                                         cols.data(), is_q.data(), (unsigned)cols.size(), fq, log_N, GEN, 1, 1, cur.p), "deep composition");
+        return compile_program(dg, dexpr.id, nbase, 1, (int)r.log_N, /*batch_inverses=*/true).bind({}, dhints, {});
+    }
 
-        // ---- FRI (fri.rs:179-249)
+    // FRI layers (fri.rs:179-249), the remainder, the proof of work, the query positions and the FRI layers' query
+    // answers; `cur` is the DEEP codeword over the LDE domain in bit-reversed order.  Returns the query positions.
+    std::vector<u64> fri_and_queries(Run &r, DeviceBuf &cur) {
+        const ProofOptions &options = r.options;
+        const int fq = r.fq, lanes = r.lanes;
+        const u64 ONE = r.ONE;
+        Proof &proof = r.proof;
         const unsigned ff = options.fri_folding_factor, log_ff = 31 - (unsigned)__builtin_clz(ff);
         struct Layer { DeviceBuf evals, leaves, nodes; Bytes root; u64 nrows; };
         std::vector<Layer> layers;
-        unsigned ln = log_N;
-        for (unsigned l = 0; l < options.fri_num_layers(N); l++) {
+        unsigned ln = r.log_N;
+        for (unsigned l = 0; l < options.fri_num_layers(r.N); l++) {
             Layer L;
             if (ln < log_ff) throw std::runtime_error("FRI: the evaluation domain is smaller than the folding factor");
             L.nrows = (u64)1 << (ln - log_ff);
@@ -273,8 +694,8 @@ public:
             L.nodes = DeviceBuf(ctx, L.nrows * 32);
             L.root.resize(32);
             ck(ctx, ms_merkle_commit_rows_sha256(ctx, cur.p, ff * lanes, L.nrows, L.leaves.p, L.nodes.p, L.root.data()), "fri layer commit");
-            coin.reseed_with_digest(L.root);
-            const Fq alpha = coin.draw();
+            r.coin.reseed_with_digest(L.root);
+            const Fq alpha = r.coin.draw();
             const u64 aw[3] = {to_mont(alpha.c[0]), to_mont(alpha.c[1]), to_mont(alpha.c[2])};
             DeviceBuf nxt(ctx, L.nrows * lanes * 8);
             ck(ctx, ms_fri_fold(ctx, fq, cur.p, ln, log_ff, ONE, aw, nxt.p), "fri fold");
@@ -289,45 +710,23 @@ public:
             ck(ctx, ms_ntt_batch(ctx, fq, cur.p, rem_size, 1, ln, MS_NTT_INVERSE, ONE), "remainder iNTT");
             std::vector<u64> w(rem_size * lanes);
             ck(ctx, ms_copy(ctx, w.data(), cur.p, w.size() * 8), "remainder download");
-            const u64 keep = rem_size / beta;
+            const u64 keep = rem_size / options.lde_blowup_factor;
             for (u64 i = 0; i < rem_size; i++) {
                 Fq v;
                 for (int l = 0; l < lanes; l++) v.c[l] = from_mont(w[i * lanes + l]);
                 if (i < keep) proof.fri_proof.remainder_coeffs.push_back(v);
                 else if (!v.is_zero()) throw std::runtime_error("FRI remainder is not low degree");
             }
-            coin.reseed_with_field_elements(proof.fri_proof.remainder_coeffs);
+            r.coin.reseed_with_field_elements(proof.fri_proof.remainder_coeffs);
         }
+        note_memory();
         // ---- proof of work + queries
         if (options.grinding_factor) {
-            ck(ctx, ms_pow_grind_sha256(ctx, coin.seed.data(), options.grinding_factor, &proof.pow_nonce), "pow");
-            if (!coin.verify_proof_of_work(options.grinding_factor, proof.pow_nonce)) throw std::runtime_error("bad nonce");
-            coin.reseed_with_int(proof.pow_nonce);
+            ck(ctx, ms_pow_grind_sha256(ctx, r.coin.seed.data(), options.grinding_factor, &proof.pow_nonce), "pow");
+            if (!r.coin.verify_proof_of_work(options.grinding_factor, proof.pow_nonce)) throw std::runtime_error("bad nonce");
+            r.coin.reseed_with_int(proof.pow_nonce);
         }
-        const std::vector<u64> positions = coin.draw_queries(options.num_queries, N);
-        auto view_of = [&](const DeviceBuf &leaves, const DeviceBuf &nodes, u64 nleaves, const std::vector<u64> &idx) {
-            const unsigned height = 63 - (unsigned)__builtin_clzll(nleaves);
-            std::vector<u8> init(idx.size() * 32), sib(idx.size() * 32), path(idx.size() * (height ? height : 1) * 32);
-            unsigned counts[3];
-            ck(ctx, ms_merkle_prove_sha256(ctx, leaves.p, nodes.p, nleaves, idx.data(), (unsigned)idx.size(), init.data(), sib.data(), path.data(), counts),
-               "merkle prove");
-            MerkleView v;
-            auto take = [](const std::vector<u8> &b, unsigned k) { std::vector<Bytes> o; for (unsigned i = 0; i < k; i++) o.emplace_back(b.begin() + 32 * i, b.begin() + 32 * i + 32); return o; };
-            v.initial_leaves = take(init, counts[0]);
-            v.sibling_leaves = take(sib, counts[1]);
-            v.nodes = take(path, counts[2]);
-            v.height = height;
-            return v;
-        };
-        auto canon_vec = [&](const std::vector<u64> &w, int l) {
-            std::vector<Fq> o;
-            for (size_t i = 0; i < w.size(); i += l) {
-                Fq v;
-                for (int k = 0; k < l; k++) v.c[k] = from_mont(w[i + k]);
-                o.push_back(v);
-            }
-            return o;
-        };
+        const std::vector<u64> positions = r.coin.draw_queries(options.num_queries, r.N);
         std::vector<u64> folded = positions;
         for (Layer &L : layers) {
             std::set<u64> s;
@@ -341,21 +740,7 @@ public:
             lp.commitment = L.root;
             proof.fri_proof.layers.push_back(std::move(lp));
         }
-        std::vector<u64> brow(positions.size() * nbase), crow(positions.size() * ce * lanes);
-        ck(ctx, ms_gather_rows(ctx, MS_FIELD_FP, base_lde.p, N, nbase, N, positions.data(), (unsigned)positions.size(), brow.data()), "base rows");
-        ck(ctx, ms_gather_rows(ctx, fq, comp_lde.p, N, (unsigned)ce, N, positions.data(), (unsigned)positions.size(), crow.data()), "composition rows");
-        proof.trace_queries.base_trace_values = canon_vec(brow, 1);
-        proof.trace_queries.composition_trace_values = canon_vec(crow, lanes);
-        if (next) {
-            std::vector<u64> erow(positions.size() * next * lanes);
-            ck(ctx, ms_gather_rows(ctx, fq, ext_lde.p, N, next, N, positions.data(), (unsigned)positions.size(), erow.data()), "extension rows");
-            proof.trace_queries.extension_trace_values = canon_vec(erow, lanes);
-            proof.trace_queries.has_extension = true;
-            proof.trace_queries.extension_trace_proof = view_of(ext_leaves, ext_nodes, N, positions);
-        }
-        proof.trace_queries.base_trace_proof = view_of(base_leaves, base_nodes, N, positions);
-        proof.trace_queries.composition_trace_proof = view_of(comp_leaves, comp_nodes, N, positions);
-        return proof;
+        return positions;
     }
 };
 
@@ -379,22 +764,11 @@ inline Bytes claim_bytes(const std::string &source, const Bytes &input, const By
 // per-row factors that are pointwise expressions of the base row (fused evaluator over the resident trace + eight 0/1
 // helper columns derived from the integer rows), then one ms_scan_affine.  instr_initial / mem_initial: the two
 // permutation start values (the reference draws them from ark_std::test_rng()).
-inline DeviceBuf device_extension(ms_ctx *ctx, const VmTrace &t, const u64 *base_dev, const std::vector<Fq> &ch, const Fq &instr_initial,
-                                  const Fq &mem_initial) {
-    const u64 n = t.n;
+// d_aux: the eight helper columns ((8, n) Montgomery words on the device) of BrainfuckTrace.helper_columns().
+inline DeviceBuf device_extension(ms_ctx *ctx, u64 n, const DeviceBuf &d_aux, const u64 *base_dev, const std::vector<Fq> &ch,
+                                  const Fq &instr_initial, const Fq &mem_initial) {
     const unsigned log_n = 63 - (unsigned)__builtin_clzll(n);
     const u64 ONE = to_mont(1);
-    // helper columns (Montgomery words)
-    std::vector<u64> aux(8 * n);
-    for (u64 r = 0; r < n; r++) {
-        const u64 ci = t.at(CURR_INSTR, r), nxt_mv = t.at(MEM_VAL, (r + 1) % n), iip = t.at(I_IP, r);
-        const bool same_ip = r > 0 && iip == t.at(I_IP, r - 1);
-        const u64 v[8] = {ci != 0, ci == ',', ci == ',' ? nxt_mv : 0, ci == '.', ci == '.' ? nxt_mv : 0, t.at(M_DUMMY, r) == 0,
-                          (u64)(t.at(I_CURR_INSTR, r) != 0 && same_ip), (u64)!same_ip};
-        for (int k = 0; k < 8; k++) aux[(u64)k * n + r] = to_mont(v[k]);
-    }
-    DeviceBuf d_aux(ctx, aux.size() * 8);
-    ck(ctx, ms_copy(ctx, d_aux.p, aux.data(), aux.size() * 8), "helper columns upload");
     std::vector<const void *> cols;
     std::vector<int> is_q(25, 0);
     for (u32 c = 0; c < 17; c++) cols.push_back(base_dev + (u64)c * n);
@@ -436,6 +810,125 @@ inline DeviceBuf device_extension(ms_ctx *ctx, const VmTrace &t, const u64 *base
     scan(8, zero3, nullptr, delta.data(), base_dev + (u64)OUT_VALUE * n, MS_FIELD_FP, 1);
     ck(ctx, ms_ctx_sync(ctx), "extension sync");       // the factor buffers above are freed when their scopes end
     return ext;
+}
+
+// the helper columns computed on the host from the integer rows of a host trace
+inline DeviceBuf device_extension(ms_ctx *ctx, const VmTrace &t, const u64 *base_dev, const std::vector<Fq> &ch, const Fq &instr_initial,
+                                  const Fq &mem_initial) {
+    const u64 n = t.n;
+    std::vector<u64> aux(8 * n);    // Montgomery words
+    for (u64 r = 0; r < n; r++) {
+        const u64 ci = t.at(CURR_INSTR, r), nxt_mv = t.at(MEM_VAL, (r + 1) % n), iip = t.at(I_IP, r);
+        const bool same_ip = r > 0 && iip == t.at(I_IP, r - 1);
+        const u64 v[8] = {ci != 0, ci == ',', ci == ',' ? nxt_mv : 0, ci == '.', ci == '.' ? nxt_mv : 0, t.at(M_DUMMY, r) == 0,
+                          (u64)(t.at(I_CURR_INSTR, r) != 0 && same_ip), (u64)!same_ip};
+        for (int k = 0; k < 8; k++) aux[(u64)k * n + r] = to_mont(v[k]);
+    }
+    DeviceBuf d_aux(ctx, aux.size() * 8);
+    ck(ctx, ms_copy(ctx, d_aux.p, aux.data(), aux.size() * 8), "helper columns upload");
+    return device_extension(ctx, n, d_aux, base_dev, ch, instr_initial, mem_initial);
+}
+
+// the helper columns computed on the device from the filled base matrix (ms_bf_helper_columns), as for a device trace
+inline DeviceBuf device_extension(ms_ctx *ctx, u64 n, const u64 *base_dev, const std::vector<Fq> &ch, const Fq &instr_initial,
+                                  const Fq &mem_initial) {
+    if (!ms_bf_helper_columns) throw std::runtime_error("the library lacks ms_bf_helper_columns (ministark_bf.h)");
+    DeviceBuf d_aux(ctx, (size_t)8 * n * 8);
+    ck(ctx, ms_bf_helper_columns(ctx, base_dev, n, d_aux.p), "helper columns");
+    return device_extension(ctx, n, d_aux, base_dev, ch, instr_initial, mem_initial);
+}
+
+// The trace of one run with its 17 base columns on the device (ministark_b200/examples/brainfuck.py::simulate with a
+// device): the VM on the host (ms_bf_run), its records uploaded, the table lengths (ms_bf_trace_sizes) and the tables
+// (ms_bf_trace_fill).  The matrix is complete when this returns.  VM errors (the memory pointer leaves the tape, the input
+// runs out, max_cycles cycles do not end the program) throw std::runtime_error with the library's message.
+struct DeviceTrace {
+    DeviceBuf base;                 // (17, n) column-major Montgomery words
+    u64 n = 0;
+    Bytes output;
+};
+inline DeviceTrace simulate_device(ms_ctx *ctx, const std::string &source, const Bytes &input = {}, u64 max_cycles = (u64)1 << 26) {
+    if (!ms_bf_run || !ms_bf_trace_sizes || !ms_bf_trace_fill) throw std::runtime_error("the library lacks the brainfuck trace (ministark_bf.h)");
+    std::vector<uint32_t> program;
+    for (u64 w : compile(source)) program.push_back((uint32_t)w);
+    // room for the longest run; pages the run does not reach are never touched
+    std::unique_ptr<uint64_t[]> log(new uint64_t[max_cycles + 1]);
+    std::unique_ptr<uint8_t[]> out(new uint8_t[max_cycles ? max_cycles : 1]);
+    uint64_t counts[2] = {0, 0};
+    if (ms_bf_run(program.data(), program.size(), input.data(), input.size(), max_cycles, log.get(), out.get(), counts) != MS_OK)
+        throw std::runtime_error(ms_last_error(nullptr));
+    const size_t nrec = counts[0] + 1;
+    DeviceTrace t;
+    t.output.assign(out.get(), out.get() + counts[1]);
+    DeviceBuf d_prog(ctx, program.size() * 4), d_log(ctx, nrec * 8);
+    ck(ctx, ms_copy(ctx, d_prog.p, program.data(), program.size() * 4), "program upload");
+    ck(ctx, ms_copy(ctx, d_log.p, log.get(), nrec * 8), "records upload");
+    uint64_t sizes[MS_BF_NSIZES];
+    ck(ctx, ms_bf_trace_sizes(ctx, static_cast<const uint32_t *>(d_prog.p), program.size(), d_log.words(), nrec, sizes), "trace sizes");
+    t.n = sizes[MS_BF_N];
+    t.base = DeviceBuf(ctx, (size_t)17 * t.n * 8);
+    DeviceBuf work(ctx, sizes[MS_BF_WORK_BYTES]);
+    ck(ctx, ms_bf_trace_fill(ctx, static_cast<const uint32_t *>(d_prog.p), program.size(), d_log.words(), nrec, sizes, work.p, t.base.p),
+       "trace fill");
+    ck(ctx, ms_ctx_sync(ctx), "trace sync");    // the fill is done before its inputs are freed and the matrix handed over
+    return t;
+}
+
+// ---- ark_std::test_rng(): ChaCha12 seeded as the reference seeds it, Fq3 elements drawn as Fq3::rand draws them
+// (ministark_b200/examples/brainfuck.py::test_rng_fq3).  The reference takes the two permutation start values of the
+// extension columns from it.
+inline void chacha_block(const uint32_t key[8], u64 counter, uint32_t out[16], int rounds = 12) {
+    uint32_t st[16] = {0x61707865, 0x3320646E, 0x79622D32, 0x6B206574};
+    for (int i = 0; i < 8; i++) st[4 + i] = key[i];
+    st[12] = (uint32_t)counter;
+    st[13] = (uint32_t)(counter >> 32);
+    st[14] = st[15] = 0;          // rand_chacha: 64-bit block counter in words 12-13, stream id 0 in words 14-15
+    uint32_t w[16];
+    for (int i = 0; i < 16; i++) w[i] = st[i];
+    auto rot = [](uint32_t v, int r) { return (v << r) | (v >> (32 - r)); };
+    auto qr = [&](int a, int b, int c, int d) {
+        w[a] += w[b]; w[d] = rot(w[d] ^ w[a], 16);
+        w[c] += w[d]; w[b] = rot(w[b] ^ w[c], 12);
+        w[a] += w[b]; w[d] = rot(w[d] ^ w[a], 8);
+        w[c] += w[d]; w[b] = rot(w[b] ^ w[c], 7);
+    };
+    for (int i = 0; i < rounds / 2; i++) {
+        qr(0, 4, 8, 12); qr(1, 5, 9, 13); qr(2, 6, 10, 14); qr(3, 7, 11, 15);
+        qr(0, 5, 10, 15); qr(1, 6, 11, 12); qr(2, 7, 8, 13); qr(3, 4, 9, 14);
+    }
+    for (int i = 0; i < 16; i++) out[i] = w[i] + st[i];
+}
+inline std::vector<Fq> test_rng_fq3(size_t count) {
+    const uint8_t seed[32] = {1, 0, 0, 0, 23, 0, 0, 0, 200, 1, 0, 0, 210, 30, 0, 0};
+    uint32_t key[8];
+    for (int i = 0; i < 8; i++) key[i] = (uint32_t)seed[4 * i] | (uint32_t)seed[4 * i + 1] << 8 | (uint32_t)seed[4 * i + 2] << 16 | (uint32_t)seed[4 * i + 3] << 24;
+    std::vector<uint32_t> words;
+    u64 ctr = 0;
+    size_t at = 0;
+    auto next_u64 = [&]() {
+        if (words.size() - at < 2) {
+            words.erase(words.begin(), words.begin() + at);
+            at = 0;
+            uint32_t blk[16];
+            chacha_block(key, ctr++, blk);
+            words.insert(words.end(), blk, blk + 16);
+        }
+        const u64 lo = words[at], hi = words[at + 1];
+        at += 2;
+        return hi << 32 | lo;
+    };
+    auto fp = [&]() {
+        for (;;) {
+            const u64 w = next_u64();
+            if (w < P) return from_mont(w);     // a raw u64 below p is taken as the Montgomery word
+        }
+    };
+    std::vector<Fq> out;
+    for (size_t i = 0; i < count; i++) {
+        const u64 c0 = fp(), c1 = fp(), c2 = fp();
+        out.push_back(Fq(c0, c1, c2));
+    }
+    return out;
 }
 
 }  // namespace bf

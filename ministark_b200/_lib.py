@@ -13,6 +13,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h"
 STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
+DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -86,6 +87,11 @@ _BF_SIGS = {
     "ms_bf_helper_columns": (ci, [vp, vp, sz, vp]),
 }
 
+# include/ministark_device.h: free device memory, for sizing a proof before anything is allocated
+_DEVICE_SIGS = {
+    "ms_device_memory": (ci, [vp, C.POINTER(sz), C.POINTER(sz)]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -116,6 +122,7 @@ def load():
         bind(lib, _STREAM_SIGS)
         bind(lib, _CHECK_SIGS)
         bind(lib, _BF_SIGS)
+        bind(lib, _DEVICE_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -1,6 +1,7 @@
 // api_core.cu — context, memory, staging and small utility kernels behind the C ABI.
 #include <cstring>
 
+#include "../../include/ministark_device.h"
 #include "ctx.cuh"
 
 namespace ms {
@@ -268,6 +269,15 @@ int ms_alloc_device(ms_ctx *c, size_t bytes, void **out) {
         cudaGetLastError();
         return fail(c, MS_ERR_NOMEM, "cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
     }
+    return MS_OK;
+}
+int ms_device_memory(ms_ctx *c, size_t *free_bytes, size_t *total_bytes) {
+    if (!c) return MS_ERR_INVALID;
+    cudaSetDevice(c->device);
+    size_t f = 0, t = 0;
+    MS_CUDA(c, cudaMemGetInfo(&f, &t));
+    if (free_bytes) *free_bytes = f;
+    if (total_bytes) *total_bytes = t;
     return MS_OK;
 }
 int ms_alloc_host_pinned(ms_ctx *c, size_t bytes, void **out) {
