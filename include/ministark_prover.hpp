@@ -3,15 +3,17 @@
 // (prover.rs:56-72) through a device-side column builder; bf::device_extension below builds the nine brainfuck
 // extension columns from the resident base trace with the fused evaluator + ms_scan_affine.
 //
-// Two residencies, chosen per proof as GpuProver (prover.py) chooses them: resident keeps every LDE matrix and tree in
+// Three residencies, chosen per proof as GpuProver (prover.py) chooses them: resident keeps every LDE matrix and tree in
 // device memory; streamed keeps the coefficients and the tree node heaps and recomputes one coset block of the LDE at a
-// time (commitment, constraint evaluation, DEEP), answering queries from the coefficients.  Both emit the same bytes.
+// time (commitment, constraint evaluation, DEEP), answering queries from the coefficients; streamed_host is streamed with
+// the node heaps in pinned host memory (ministark_host_nodes.h).  All emit the same bytes.
 //
 // Host logic (coin, AIR, programs, wire format) comes from ministark_host.hpp and is CPU-tested.  This file only strings
 // the ms_* calls together; linked against the CPU build of the ABI it is byte-compared with the CPU restatement of the
 // reference prover, and on a GPU with the Python driver (tests/test_zz_gpu_cpp_prover.py,
 // tests/test_gpu_cpp_stream_prover.py).
 #pragma once
+#include <chrono>
 #include <cstdio>
 #include <memory>
 #include <stdexcept>
@@ -21,6 +23,7 @@
 #include "ministark_device.h"
 #include "ministark_examples.hpp"
 #include "ministark_host.hpp"
+#include "ministark_host_nodes.h"
 #include "ministark_stream.h"
 
 // ministark_b200.h is the ABI every library build exports.  The entry points of the headers beside it are referenced
@@ -30,6 +33,7 @@
 #pragma weak ms_device_memory
 #pragma weak ms_merkle_commit_block_sha256
 #pragma weak ms_lde_rows
+#pragma weak ms_merkle_commit_block_sha256_host
 #pragma weak ms_bf_run
 #pragma weak ms_bf_trace_sizes
 #pragma weak ms_bf_trace_fill
@@ -117,9 +121,10 @@ inline Expr deep_expression(Graph &g, const std::vector<std::pair<u64, int64_t>>
 // context's scratch arenas (prover.py MEMORY_RESERVE).
 constexpr u64 MEMORY_RESERVE = (u64)3 << 30;
 
-struct PeakBytes { u64 resident, streamed; };
+// device bytes of each residency, and the pinned host bytes of streamed_host (its node heaps)
+struct PeakBytes { u64 resident, streamed, streamed_host, host; };
 
-// Peak device bytes of one proof in each residency, from the shapes (prover.py peak_bytes).  lanes: 1 for Fq = Fp, 3 for
+// Peak bytes of one proof in each residency, from the shapes (prover.py peak_bytes).  lanes: 1 for Fq = Fp, 3 for
 // Fq3; ce_blowup: the composition blow-up; ff: the FRI folding factor.
 inline PeakBytes peak_bytes(u64 n, u64 beta, u64 nbase, u64 next, u64 lanes, u64 ce_blowup, u64 ff = 2) {
     const u64 N = n * beta, M = n * ce_blowup;
@@ -127,7 +132,8 @@ inline PeakBytes peak_bytes(u64 n, u64 beta, u64 nbase, u64 next, u64 lanes, u64
     const u64 ntrees = next ? 3 : 2;
     const u64 fri = (8 * lanes + 64) * N / (ff - 1);
     const u64 common = 8 * words * n + 8 * N * lanes + fri + ((u64)16 << 20);
-    return {common + 8 * M * lanes + 8 * words * N + 64 * ntrees * N, common + 8 * words * n + 32 * ntrees * N + 32 * n};
+    const u64 blocks = common + 8 * words * n + 32 * n;
+    return {common + 8 * M * lanes + 8 * words * N + 64 * ntrees * N, blocks + 32 * ntrees * N, blocks + 64 * n, 32 * ntrees * N};
 }
 
 inline std::string gib(long double b) {
@@ -183,21 +189,43 @@ inline MerkleWalk merkle_walk(u64 n_leaves, const std::vector<u64> &indices) {
     return w;
 }
 
+// Where node i of a tree committed in 2^log_b blocks lives in the split heap of ministark_host_nodes.h (cosets.py
+// heap_location): block -1 and index i in the top heap of 2 * 2^log_b digests, else the block and the index in its local
+// heap.
+struct HeapLocation { int64_t block; u64 index; };
+inline HeapLocation heap_location(u64 i, unsigned log_b) {
+    const u64 beta = (u64)1 << log_b;
+    if (i < 2 * beta) return {-1, i};
+    const unsigned d = 63 - (unsigned)__builtin_clzll(i) - log_b;
+    return {(int64_t)((i >> d) - beta), ((u64)1 << d) | (i & (((u64)1 << d) - 1))};
+}
+
 class GpuProver {
     ms_ctx *ctx = nullptr;
+    void *pinned = nullptr;     // streamed_host's node heaps (ms_alloc_host_pinned), kept for the next proof
+    u64 pinned_size = 0;
 
 public:
     // bytes one proof may use on the device; 0: whatever the device has free
     u64 memory_budget = 0;
-    // "resident" or "streamed": what the last proof ran (empty before the first)
+    // pinned host bytes one proof may hold (streamed_host's node heaps); 0: none.  Heaps pinned under a larger budget are
+    // freed when the next proof starts.
+    u64 host_memory_budget = 0;
+    // "resident", "streamed" or "streamed_host": what the last proof ran (empty before the first)
     std::string last_residency;
     // the lowest free device memory ms_device_memory reported between the phases of the last proof
     u64 lowest_free_bytes = 0;
+    // seconds the last proof spent pinning host memory (0 when it reused the held heaps or needed none)
+    double last_pin_seconds = 0;
 
     explicit GpuProver(int device = 0) {
         if (ms_ctx_create(device, &ctx) != MS_OK) throw std::runtime_error("ms_ctx_create failed (no CUDA device? there is no CPU fallback)");
     }
-    ~GpuProver() { if (ctx) ms_ctx_destroy(ctx); }
+    ~GpuProver() {
+        if (!ctx) return;
+        release_host_memory();
+        ms_ctx_destroy(ctx);
+    }
     GpuProver(const GpuProver &) = delete;
     GpuProver &operator=(const GpuProver &) = delete;
 
@@ -220,13 +248,30 @@ public:
         const int64_t avail = (f >= (u64)INT64_MAX ? INT64_MAX : (int64_t)f) - (int64_t)MEMORY_RESERVE;
         return memory_budget ? std::min<int64_t>((int64_t)memory_budget, avail) : avail;
     }
-    // "resident" if its estimate fits, else "streamed" if that fits, else the refusal (nothing is allocated yet)
+    // "resident" if its estimate fits, else "streamed" if that fits, else "streamed_host" if its device estimate fits and
+    // its node heaps fit host_memory_budget, else the refusal (nothing is allocated yet)
     std::string choose_residency(const PeakBytes &est) const {
         const int64_t budget = memory_available();
         if ((int64_t)est.resident <= budget) return "resident";
         if ((int64_t)est.streamed <= budget) return "streamed";
-        throw std::runtime_error("the proof does not fit on the device: it needs about " + gib(est.resident) + " resident or " +
-                                 gib(est.streamed) + " streamed, and " + gib(budget) + " is available");
+        if (host_memory_budget && (int64_t)est.streamed_host <= budget && est.host <= host_memory_budget) return "streamed_host";
+        std::string msg = "the proof does not fit on the device: it needs about " + gib(est.resident) + " resident or " +
+                          gib(est.streamed) + " streamed, and " + gib(budget) + " is available";
+        if (host_memory_budget)
+            msg += "; with the Merkle node heaps in pinned host memory it needs about " + gib(est.streamed_host) + " on the device and " +
+                   gib(est.host) + " of host memory, and " + gib(host_memory_budget) + " of host memory is allowed";
+        throw std::runtime_error(msg);
+    }
+
+    // pinned host memory held for streamed_host's node heaps (0 before its first such proof)
+    u64 pinned_bytes() const { return pinned_size; }
+    // frees the pinned node heaps; the next streamed_host proof pins them again
+    void release_host_memory() {
+        if (!pinned) return;
+        ms_ctx_sync(ctx);
+        ms_free(ctx, pinned);
+        pinned = nullptr;
+        pinned_size = 0;
     }
 
     // base_trace: num_base_columns x n Montgomery words, column-major, HOST memory.  public_inputs: handed to gen_hints;
@@ -261,6 +306,7 @@ private:
         u32 nbase, next;
         const u64 *host_trace;      // exactly one of host_trace / device_trace holds the base trace
         DeviceBuf &device_trace;
+        u8 *host_heaps = nullptr;   // streamed_host: the node heaps of the trees, N x 32 B each, in commitment order
     };
 
     void note_memory() { lowest_free_bytes = std::min<u64>(lowest_free_bytes, free_memory()); }
@@ -289,13 +335,30 @@ private:
         r.log_ce = r.log_n + (63 - (unsigned)__builtin_clzll(r.ce));
         r.proof.options = options;
         r.proof.trace_len = n;
-        last_residency = choose_residency(peak_bytes(n, beta, r.nbase, next, lanes, r.ce, options.fri_folding_factor));
+        const PeakBytes est = peak_bytes(n, beta, r.nbase, next, lanes, r.ce, options.fri_folding_factor);
+        if (pinned_size > host_memory_budget) release_host_memory();   // heaps pinned under a larger budget are not held past a lower one
+        last_residency = choose_residency(est);
+        last_pin_seconds = 0;
         lowest_free_bytes = UINT64_MAX;
         note_memory();
+        if (last_residency == "streamed_host") r.host_heaps = host_heaps(est.host);
         if (last_residency == "resident") prove_resident(r);
         else prove_streamed(r);
         note_memory();
         return std::move(r.proof);
+    }
+
+    // at least `bytes` of pinned host memory: the held allocation while it is large enough
+    u8 *host_heaps(u64 bytes) {
+        if (!ms_merkle_commit_block_sha256_host) throw std::runtime_error("the library lacks the host node heaps (ministark_host_nodes.h)");
+        if (pinned_size < bytes) {
+            release_host_memory();
+            const auto t0 = std::chrono::steady_clock::now();
+            ck(ctx, ms_alloc_host_pinned(ctx, bytes, &pinned), "ms_alloc_host_pinned");
+            pinned_size = bytes;
+            last_pin_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        }
+        return static_cast<u8 *>(pinned);
     }
 
     // the base trace on the device: the handed-over device matrix, or a fresh upload of the host one
@@ -420,28 +483,53 @@ private:
         ck(ctx, ms_set_option(ctx, "drop_plans", 1), "drop_plans");
     }
 
+    // a tree's node heap: whole on the device, or split (ministark_host_nodes.h) into the top heap here and the blocks'
+    // local heaps in pinned host memory
+    struct NodeHeap {
+        DeviceBuf dev;
+        std::vector<u8> top;
+        const u8 *host = nullptr;
+    };
+
     // Merkle commitment of the bit-reversed LDE of `polys`, one coset block at a time: block q is transformed into `blk`
     // and hashed into its subtree of the node heap; the top log_b levels come from the block roots.  Returns the node heap
-    // and writes the root.
-    DeviceBuf commit_blocks(Run &r, const void *polys, void *blk, int field, unsigned ncols, const std::vector<u64> &offsets, Bytes &root) {
+    // and writes the root.  With host_heap (N x 32 B pinned), block q's subtree is the local heap at host_heap + q * n * 32.
+    NodeHeap commit_blocks(Run &r, const void *polys, void *blk, int field, unsigned ncols, const std::vector<u64> &offsets, Bytes &root,
+                           u8 *host_heap = nullptr) {
         const u64 beta = (u64)1 << r.log_b;
-        DeviceBuf nodes(ctx, r.N * 32), roots(ctx, beta * 32);
+        DeviceBuf nodes(ctx, (host_heap ? 2 * beta : r.N) * 32), own_roots;
+        u8 *roots = static_cast<u8 *>(nodes.p) + 32 * beta;          // the top heap's last level
+        if (!host_heap) {
+            own_roots = DeviceBuf(ctx, beta * 32);
+            roots = static_cast<u8 *>(own_roots.p);
+        }
         for (u64 q = 0; q < beta; q++) {
             lde_block(polys, blk, field, ncols, r.log_n, offsets[q]);
-            ck(ctx, ms_merkle_commit_block_sha256(ctx, field, blk, r.n, ncols, r.log_n, r.log_b, q, nodes.p, static_cast<u8 *>(roots.p) + 32 * q),
-               "block commit");
+            if (host_heap)
+                ck(ctx, ms_merkle_commit_block_sha256_host(ctx, field, blk, r.n, ncols, r.log_n, host_heap + q * r.n * 32, roots + 32 * q),
+                   "block commit (host heap)");
+            else
+                ck(ctx, ms_merkle_commit_block_sha256(ctx, field, blk, r.n, ncols, r.log_n, r.log_b, q, nodes.p, roots + 32 * q), "block commit");
         }
-        if (beta > 1) ck(ctx, ms_merkle_nodes_sha256(ctx, roots.p, beta, nodes.p), "block roots");
+        if (beta > 1) ck(ctx, ms_merkle_nodes_sha256(ctx, roots, beta, nodes.p), "block roots");
         const u8 zero[32] = {0};          // the unused default digest (named by a walk over a 2-leaf tree)
         ck(ctx, ms_copy(ctx, nodes.p, zero, 32), "node 0");
         root.resize(32);
         ck(ctx, ms_copy(ctx, root.data(), static_cast<u8 *>(nodes.p) + 32, 32), "root");
-        return nodes;
+        NodeHeap h;
+        if (host_heap) {
+            h.top.resize(2 * beta * 32);
+            ck(ctx, ms_copy(ctx, h.top.data(), nodes.p, h.top.size()), "top heap");
+            h.host = host_heap;
+        } else {
+            h.dev = std::move(nodes);
+        }
+        return h;
     }
 
     // the rows at `positions` and their MerkleView without the LDE: rows and leaf digests from the coefficients
-    // (ms_lde_rows), path nodes gathered from the resident node heap
-    MerkleView streamed_rows(Run &r, const void *polys, int field, unsigned ncols, const DeviceBuf &nodes, const std::vector<u64> &positions,
+    // (ms_lde_rows), path nodes gathered from the node heap (on the device, or split between here and pinned host memory)
+    MerkleView streamed_rows(Run &r, const void *polys, int field, unsigned ncols, const NodeHeap &nodes, const std::vector<u64> &positions,
                              std::vector<u64> &rows) {
         const MerkleWalk w = merkle_walk(r.N, positions);
         std::vector<u64> ids = positions;
@@ -457,9 +545,16 @@ private:
             for (size_t j = 0; j < row_words; j++) put_u64_le(ser, from_mont(all[k * row_words + j]));
             (k < positions.size() + w.init.size() ? v.initial_leaves : v.sibling_leaves).push_back(sha256({ser}));
         }
-        if (!w.path.empty()) {
+        if (!w.path.empty() && nodes.host) {
+            ck(ctx, ms_ctx_sync(ctx), "sync");    // the last subtrees' copies to host memory
+            for (u64 i : w.path) {
+                const HeapLocation at = heap_location(i, r.log_b);
+                const u8 *d = at.block < 0 ? nodes.top.data() + 32 * at.index : nodes.host + ((u64)at.block * r.n + at.index) * 32;
+                v.nodes.emplace_back(d, d + 32);
+            }
+        } else if (!w.path.empty()) {
             std::vector<u8> path(w.path.size() * 32);
-            ck(ctx, ms_gather_rows_rowmajor(ctx, nodes.p, 4, r.N, w.path.data(), (unsigned)w.path.size(), path.data()), "path nodes");
+            ck(ctx, ms_gather_rows_rowmajor(ctx, nodes.dev.p, 4, r.N, w.path.data(), (unsigned)w.path.size(), path.data()), "path nodes");
             for (size_t i = 0; i < w.path.size(); i++) v.nodes.emplace_back(path.begin() + 32 * i, path.begin() + 32 * i + 32);
         }
         v.height = r.log_N;
@@ -474,24 +569,26 @@ private:
         Proof &proof = r.proof;
         if (!ms_merkle_commit_block_sha256 || !ms_lde_rows) throw std::runtime_error("the library lacks the streamed residency (ministark_stream.h)");
         const std::vector<u64> offsets = coset_offsets(log_n, r.log_b);
+        auto host_heap = [&](u64 tree) { return r.host_heaps ? r.host_heaps + tree * N * 32 : nullptr; };   // streamed_host
 
         // ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
         DeviceBuf d_trace = device_base(r), base_polys(ctx, (size_t)nbase * n * 8), base_blk(ctx, (size_t)nbase * n * 8);
         ck(ctx, ms_ntt_batch_to(ctx, MS_FIELD_FP, d_trace.p, n, base_polys.p, n, nbase, log_n, MS_NTT_INVERSE, ONE), "interpolate");
-        DeviceBuf base_nodes = commit_blocks(r, base_polys.p, base_blk.p, MS_FIELD_FP, nbase, offsets, proof.base_trace_commitment);
+        NodeHeap base_nodes = commit_blocks(r, base_polys.p, base_blk.p, MS_FIELD_FP, nbase, offsets, proof.base_trace_commitment, host_heap(0));
         r.coin.reseed_with_digest(proof.base_trace_commitment);
         note_memory();
 
         // ---- extension trace commitment
         std::vector<Fq> challenges, hints;
         DeviceBuf ext = extension_columns(r, d_trace, challenges, hints);
-        DeviceBuf ext_polys, ext_blk, ext_nodes;
+        DeviceBuf ext_polys, ext_blk;
+        NodeHeap ext_nodes;
         if (next) {
             ext_polys = DeviceBuf(ctx, (size_t)next * n * lanes * 8);
             ck(ctx, ms_ntt_batch_to(ctx, fq, ext.p, n, ext_polys.p, n, next, log_n, MS_NTT_INVERSE, ONE), "extension interpolate");
             ext.release();
             ext_blk = DeviceBuf(ctx, (size_t)next * n * lanes * 8);
-            ext_nodes = commit_blocks(r, ext_polys.p, ext_blk.p, fq, next, offsets, proof.extension_trace_commitment);
+            ext_nodes = commit_blocks(r, ext_polys.p, ext_blk.p, fq, next, offsets, proof.extension_trace_commitment, host_heap(1));
             proof.has_extension = true;
             r.coin.reseed_with_digest(proof.extension_trace_commitment);
         }
@@ -535,7 +632,8 @@ private:
         const void *comp_polys = ce > 1 ? comp_split.p : comp_evals.p;
         ck(ctx, ms_set_option(ctx, "drop_scratch", 1), "drop_scratch");   // the size-M transform's temporary
         DeviceBuf comp_blk(ctx, ce * n * lanes * 8);
-        DeviceBuf comp_nodes = commit_blocks(r, comp_polys, comp_blk.p, fq, (unsigned)ce, offsets, proof.composition_trace_commitment);
+        NodeHeap comp_nodes = commit_blocks(r, comp_polys, comp_blk.p, fq, (unsigned)ce, offsets, proof.composition_trace_commitment,
+                                            host_heap(next ? 2 : 1));
         r.coin.reseed_with_digest(proof.composition_trace_commitment);
         note_memory();
 

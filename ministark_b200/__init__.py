@@ -149,6 +149,11 @@ class Context:
         self._ck(self.lib.ms_alloc_device(self.h, nbytes, C.byref(out)))
         return int(out.value)
 
+    def alloc_host_pinned(self, nbytes):
+        out = C.c_void_p()
+        self._ck(self.lib.ms_alloc_host_pinned(self.h, nbytes, C.byref(out)))
+        return int(out.value)
+
     def free(self, ptr):
         self._ck(self.lib.ms_free(self.h, ptr))
 
@@ -212,6 +217,13 @@ class Context:
         col_stride = (1 << log_block_rows) if col_stride is None else col_stride
         self._ck(self.lib.ms_merkle_commit_block_sha256(self.h, field, _ptr(cols), col_stride, ncols, log_block_rows,
                                                         log_blocks, block, _ptr(nodes), _ptr(block_root)))
+
+    def merkle_commit_block_host(self, cols, field, log_block_rows, ncols, host_subtree, block_root, col_stride=None):
+        """hash one coset block (2^log_block_rows rows at `cols`) and copy its local heap to `host_subtree` (pinned host
+        memory, 2^log_block_rows x 32 bytes; complete after sync()); the block root goes to `block_root` (32 bytes)"""
+        col_stride = (1 << log_block_rows) if col_stride is None else col_stride
+        self._ck(self.lib.ms_merkle_commit_block_sha256_host(self.h, field, _ptr(cols), col_stride, ncols, log_block_rows,
+                                                             _ptr(host_subtree), _ptr(block_root)))
 
     def lde_rows(self, coeffs, field, log_n, log_blowup, ncols, positions, offset=GENERATOR, col_stride=None, out=None):
         """rows `positions` of the bit-reversed coset LDE of `coeffs`, evaluated from the coefficients; returns

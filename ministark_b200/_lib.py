@@ -14,6 +14,7 @@ STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
+HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -92,6 +93,11 @@ _DEVICE_SIGS = {
     "ms_device_memory": (ci, [vp, C.POINTER(sz), C.POINTER(sz)]),
 }
 
+# include/ministark_host_nodes.h: block subtrees of a streamed commitment copied to pinned host memory
+_HOST_NODES_SIGS = {
+    "ms_merkle_commit_block_sha256_host": (ci, [vp, ci, vp, sz, ui, ui, vp, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -123,6 +129,7 @@ def load():
         bind(lib, _CHECK_SIGS)
         bind(lib, _BF_SIGS)
         bind(lib, _DEVICE_SIGS)
+        bind(lib, _HOST_NODES_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -38,6 +38,19 @@ def block_program(air):
     return prog
 
 
+def heap_location(i, log_b):
+    """where node i of the heap of a tree committed in 2^log_b blocks lives when the heap is split
+    (include/ministark_host_nodes.h): (None, i) in the top heap of 2 * 2^log_b digests, else (block, index in the block's
+    local heap).  Node i at level L = floor(log2 i) >= log_b + 1 is one of the 2^d, d = L - log_b, nodes block
+    (i >> d) - 2^log_b owns on that level; in the block's heap the same level starts at 1 << d."""
+    i = int(i)
+    beta = 1 << log_b
+    if i < 2 * beta:
+        return None, i
+    d = i.bit_length() - 1 - log_b
+    return (i >> d) - beta, (1 << d) | (i & ((1 << d) - 1))
+
+
 def merkle_walk(n_leaves, indices):
     """The index walk of MerkleTreeImpl::prove (src/merkle.rs:149-207; csrc/hash.cu ms_merkle_prove_sha256): which
     leaves and which heap nodes a batched proof names.  Returns (initial leaf indices, sibling leaf indices, node indices)."""

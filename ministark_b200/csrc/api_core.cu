@@ -198,6 +198,7 @@ int ms_ctx_destroy(ms_ctx *c) {
     if (!c) return MS_ERR_INVALID;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
+    ms::host_nodes_drain(c, true);
     c->plans.clear();
     for (auto &t : c->tw_tables) cudaFree(t.second);
     for (auto &e : c->ptr_tables) cudaFree(e.dev);
@@ -221,7 +222,7 @@ int ms_ctx_set_stream(ms_ctx *c, void *s) {
 int ms_ctx_sync(ms_ctx *c) {
     if (!c) return MS_ERR_INVALID;
     MS_CUDA(c, cudaStreamSynchronize(c->stream));
-    return MS_OK;
+    return ms::host_nodes_drain(c, false);     // node heaps still crossing to host memory
 }
 
 // tuning / A-B switches (process-wide): "ntt_tma" 0|1, "ntt_tma_groups" 2|3, "ntt_tma_stages" 3..8
@@ -244,10 +245,11 @@ int ms_set_option(ms_ctx *c, const char *name, int64_t value) {
         ms::ntt_drop_plans(c);
         return MS_OK;
     }
-    if (!strcmp(name, "drop_scratch")) {   // free the context's scratch arenas (regrown on demand)
+    if (!strcmp(name, "drop_scratch")) {   // free the context's scratch arenas and node staging (regrown on demand)
         if (!c) return MS_ERR_INVALID;
         cudaSetDevice(c->device);
         MS_CUDA(c, cudaStreamSynchronize(c->stream));
+        if (int rc = ms::host_nodes_drain(c, true)) return rc;
         for (ms::Scratch &s : c->scratch) {
             if (s.ptr) MS_CUDA(c, cudaFree(s.ptr));
             s.ptr = nullptr;

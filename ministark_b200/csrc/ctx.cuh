@@ -49,6 +49,12 @@ struct ms_ctx {
     std::map<std::tuple<int, unsigned, int, uint64_t, unsigned, int>, std::shared_ptr<ms::NttPlanDev>> plans;
     std::deque<ms::PtrTable> ptr_tables;       // cached device copies of LDE scatter pointer tables (deque: stable addresses)
     std::map<unsigned, ms::u64 *> tw_tables;   // log_n -> two-level g_n^e table (4096 + n/4096 words), ntt_plan_tables
+    // ms_merkle_commit_block_sha256_host: block heaps are built in node_stage[k] and copied to pinned host memory on
+    // node_copy_stream; node_copied[k] marks the end of the last copy out of node_stage[k] (created on first use)
+    cudaStream_t node_copy_stream = nullptr;
+    ms::Scratch node_stage[2];
+    cudaEvent_t node_built[2] = {nullptr, nullptr}, node_copied[2] = {nullptr, nullptr};
+    int node_stage_next = 0;
 };
 
 namespace ms {
@@ -68,6 +74,9 @@ void clear_noctx_error();
 int scratch_get(ms_ctx *c, int slot, size_t bytes, void **out);
 // true if the pointer is directly usable by kernels without crossing PCIe (device / managed)
 bool is_device_ptr(const void *p);
+// waits for the node heap copies of ms_merkle_commit_block_sha256_host; with release, also frees their staging buffers,
+// stream and events (hash.cu)
+int host_nodes_drain(ms_ctx *c, bool release);
 
 // RAII staging of a possibly-host buffer: gives a device pointer, copies in/out as asked.
 struct Staged {

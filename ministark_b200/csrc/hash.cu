@@ -15,6 +15,7 @@
 #include <cstring>
 #include "ctx.cuh"
 #include "../../include/ministark_stream.h"
+#include "../../include/ministark_host_nodes.h"
 #include <algorithm>
 #include <cstring>
 #include <deque>
@@ -315,11 +316,95 @@ static int merkle_nodes_dev(ms_ctx *c, const u32 *leaves, size_t n, u32 *nodes) 
     return MS_OK;
 }
 
+int host_nodes_drain(ms_ctx *c, bool release) {
+    if (!c->node_copy_stream) return MS_OK;
+    MS_CUDA(c, cudaStreamSynchronize(c->node_copy_stream));
+    if (!release) return MS_OK;
+    for (int k = 0; k < 2; k++) {
+        if (c->node_stage[k].ptr) MS_CUDA(c, cudaFree(c->node_stage[k].ptr));
+        c->node_stage[k] = Scratch{};
+        if (c->node_built[k]) MS_CUDA(c, cudaEventDestroy(c->node_built[k]));
+        if (c->node_copied[k]) MS_CUDA(c, cudaEventDestroy(c->node_copied[k]));
+        c->node_built[k] = c->node_copied[k] = nullptr;
+    }
+    MS_CUDA(c, cudaStreamDestroy(c->node_copy_stream));
+    c->node_copy_stream = nullptr;
+    return MS_OK;
+}
+
+// both staging buffers of ms_merkle_commit_block_sha256_host at least `bytes`, with the copy stream and the events
+static int host_nodes_staging(ms_ctx *c, size_t bytes) {
+    if (!c->node_copy_stream) {
+        MS_CUDA(c, cudaStreamCreateWithFlags(&c->node_copy_stream, cudaStreamNonBlocking));
+        for (int k = 0; k < 2; k++) {
+            MS_CUDA(c, cudaEventCreateWithFlags(&c->node_built[k], cudaEventDisableTiming));
+            MS_CUDA(c, cudaEventCreateWithFlags(&c->node_copied[k], cudaEventDisableTiming));
+        }
+    }
+    if (c->node_stage[0].cap >= bytes) return MS_OK;
+    MS_CUDA(c, cudaStreamSynchronize(c->node_copy_stream));   // no copy may still read a buffer that is replaced
+    for (Scratch &s : c->node_stage) {
+        if (s.ptr) MS_CUDA(c, cudaFree(s.ptr));
+        s = Scratch{};
+        MS_CUDA(c, cudaMalloc(&s.ptr, bytes));
+        s.cap = bytes;
+    }
+    return MS_OK;
+}
+
 }  // namespace ms
 
 using namespace ms;
 
 extern "C" {
+
+// include/ministark_host_nodes.h.  Block b's heap is built in staging buffer k = b mod 2 on the compute stream, after the
+// copy that last read that buffer (two blocks ago) has finished; the copy stream then moves it to host_subtree while the
+// compute stream goes on with the next block.
+int ms_merkle_commit_block_sha256_host(ms_ctx *c, int field, const void *cols, size_t col_stride_elems, unsigned ncols,
+                                       unsigned log_block_rows, void *host_subtree, void *block_root) {
+    if (!c || !cols || !host_subtree || !block_root) return MS_ERR_INVALID;
+    if (field != MS_FIELD_FP && field != MS_FIELD_FQ3) return fail(c, MS_ERR_INVALID, "unknown field id %d", field);
+    if (ncols == 0) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256_host: no columns");
+    if (log_block_rows > 36) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256_host: block too large");
+    const size_t nb = (size_t)1 << log_block_rows, bytes = nb * 32;
+    if (ncols > 1 && col_stride_elems < nb) return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256_host: stride < block rows");
+    cudaSetDevice(c->device);
+    // an asynchronous copy into pageable memory is staged by the driver and serialises with the compute stream.  Both ends
+    // of the range are checked, so a pinned start whose range runs past its allocation is refused too.
+    for (const char *p : {(const char *)host_subtree, (const char *)host_subtree + bytes - 1}) {
+        cudaPointerAttributes a;
+        MS_CUDA(c, cudaPointerGetAttributes(&a, p));
+        if (a.type != cudaMemoryTypeHost)
+            return fail(c, MS_ERR_INVALID, "ms_merkle_commit_block_sha256_host: the subtree buffer is %s memory, not pinned host memory",
+                        a.type == cudaMemoryTypeUnregistered ? "pageable host" : a.type == cudaMemoryTypeManaged ? "managed" : "device");
+    }
+    int rc = host_nodes_staging(c, bytes);
+    if (rc) return rc;
+    const int k = c->node_stage_next;
+    c->node_stage_next ^= 1;
+    u32 *heap = (u32 *)c->node_stage[k].ptr;
+    Staged in(c, cols, ((size_t)(ncols - 1) * col_stride_elems + nb) * field * 8, true, false);
+    if (in.rc) return in.rc;
+    void *lv;
+    if ((rc = scratch_get(c, 2, bytes, &lv))) return rc;
+    if ((rc = hash_rows_dev(c, field, in.as<u64>(), col_stride_elems, ncols, nb, (u32 *)lv))) return rc;
+    MS_CUDA(c, cudaStreamWaitEvent(c->stream, c->node_copied[k], 0));
+    const u32 *root = (const u32 *)lv;                      // one row: the root is its leaf digest, slot 0 the whole heap
+    if (nb == 1) {
+        MS_CUDA(c, cudaMemsetAsync(heap, 0, 32, c->stream));
+    } else {
+        if ((rc = merkle_nodes_dev(c, (const u32 *)lv, nb, heap))) return rc;
+        root = heap + 8;
+    }
+    MS_CUDA(c, cudaEventRecord(c->node_built[k], c->stream));
+    MS_CUDA(c, cudaStreamWaitEvent(c->node_copy_stream, c->node_built[k], 0));
+    MS_CUDA(c, cudaMemcpyAsync(host_subtree, heap, bytes, cudaMemcpyDeviceToHost, c->node_copy_stream));
+    MS_CUDA(c, cudaEventRecord(c->node_copied[k], c->node_copy_stream));
+    MS_CUDA(c, cudaMemcpyAsync(block_root, root, 32, cudaMemcpyDefault, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    return in.finish();
+}
 
 int ms_hash_rows_sha256(ms_ctx *c, int field, const void *cols, size_t col_stride_elems, unsigned ncols, size_t nrows,
                         void *digests) {

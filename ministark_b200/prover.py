@@ -20,8 +20,10 @@ torch is used for device buffers and the stream only.  There is no CPU fallback:
 Context constructor raises.
 """
 import copy
+import ctypes as C
 import hashlib
 import time
+import weakref
 
 import numpy as np
 import torch
@@ -31,7 +33,7 @@ from . import deep
 from . import expr as E
 from .air import Air
 from .channel import ProverChannel, PublicCoin, serialize_element
-from .cosets import block_program, coset_offsets, merkle_walk
+from .cosets import block_program, coset_offsets, heap_location, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
 
 P = E.P
@@ -133,20 +135,30 @@ MEMORY_RESERVE = 3 << 30
 
 
 def peak_bytes(n, beta, nbase, next_, fq, ce_blowup, ff=2):
-    """Peak device bytes of one proof in each residency, from the shapes: {"resident": .., "streamed": ..}.
+    """Peak bytes of one proof in each residency, from the shapes: {"resident": .., "streamed": .., "streamed_host": ..}
+    on the device, and "host": the pinned host bytes of streamed_host.
 
     resident: every matrix's coefficients and bit-reversed LDE, and the leaf and node arrays of every tree, live until
     the queries, and so does the ce-domain composition column.  streamed: the coefficients, one coset block of every
-    matrix and the node arrays (no leaves; one block's leaf digests in context scratch).  Both hold the DEEP codeword and the FRI
-    layers (folded codewords and trees, a geometric series in the folding factor ff), and 16 MiB for the small buffers
-    (block roots, remainder, query rows) and the allocator's rounding."""
+    matrix and the node arrays (no leaves; one block's leaf digests in context scratch).  streamed_host: streamed with the
+    node arrays in pinned host memory ("host"); the device holds two staging heaps of one block instead.  All hold the
+    DEEP codeword and the FRI layers (folded codewords and trees, a geometric series in the folding factor ff), and
+    16 MiB for the small buffers (block roots, top heaps, remainder, query rows) and the allocator's rounding."""
     N, M = n * beta, n * ce_blowup
     words = nbase + fq * (next_ + ce_blowup)                 # words per row over all matrices
     ntrees = 3 if next_ else 2
     fri = (8 * fq + 64) * N // (ff - 1)
     common = 8 * words * n + 8 * N * fq + fri + (16 << 20)
+    blocks = common + 8 * words * n + 32 * n
     return {"resident": common + 8 * M * fq + 8 * words * N + 64 * ntrees * N,
-            "streamed": common + 8 * words * n + 32 * ntrees * N + 32 * n}
+            "streamed": blocks + 32 * ntrees * N,
+            "streamed_host": blocks + 64 * n,
+            "host": 32 * ntrees * N}
+
+
+def _free_pinned(ctx, addr):
+    ctx.sync()                  # the last block heaps may still be crossing into it
+    ctx.free(addr)
 
 
 def _gib(b):
@@ -163,14 +175,20 @@ class _Run:
 class GpuProver:
     """owns the device context (one in-order stream) and runs default_prove.
 
-    Two residencies, chosen per proof from the estimates of `peak_bytes` against `memory_available()`:
-      resident   every LDE matrix and both arrays of every Merkle tree stay in HBM until the queries (the fastest);
-      streamed   only coefficients and tree nodes stay; each coset block of the LDE is recomputed where it is needed
-                 (commitment, constraint evaluation, DEEP) and query rows come from the coefficients (ms_lde_rows).
-    Both emit the same proof bytes.  The resident path runs whenever it fits."""
+    Three residencies, chosen per proof from the estimates of `peak_bytes` against `memory_available()` and
+    `host_memory_budget`:
+      resident       every LDE matrix and both arrays of every Merkle tree stay in HBM until the queries (the fastest);
+      streamed       only coefficients and tree nodes stay; each coset block of the LDE is recomputed where it is needed
+                     (commitment, constraint evaluation, DEEP) and query rows come from the coefficients (ms_lde_rows);
+      streamed_host  streamed with every tree's node heap in pinned host memory: each block's subtree is copied out
+                     while the next block's LDE runs, and the queries gather their path nodes on the host.
+    All emit the same proof bytes.  The resident path runs whenever it fits, streamed_host only with a host budget."""
     _shared = {}
     memory_budget = None        # bytes one proof may use on the device; None: whatever the device has free
-    last_residency = None       # "resident" or "streamed": what the last proof ran
+    host_memory_budget = None   # pinned host bytes one proof may hold (streamed_host's node heaps); None: none.  Heaps
+                                # pinned under a larger budget are freed when the next proof starts
+    last_residency = None       # "resident", "streamed" or "streamed_host": what the last proof ran
+    _pinned = None              # (address, bytes, finalizer) of the pinned node heaps, kept for the next proof
 
     @classmethod
     def shared(cls, device=0):
@@ -178,13 +196,35 @@ class GpuProver:
             cls._shared[device] = cls(device)
         return cls._shared[device]
 
-    def __init__(self, device=0, memory_budget=None):
+    def __init__(self, device=0, memory_budget=None, host_memory_budget=None):
         self.device = torch.device("cuda", device)
         self.stream = torch.cuda.Stream(device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self.ctx = Context(device, stream=self.stream.cuda_stream)
         self._airs = {}
         self.memory_budget = memory_budget
+        self.host_memory_budget = host_memory_budget
+
+    @property
+    def pinned_bytes(self):
+        """pinned host memory the prover holds for streamed_host's node heaps (0 before its first such proof)"""
+        return self._pinned[1] if self._pinned else 0
+
+    def release_host_memory(self):
+        """free the pinned node heaps; the next streamed_host proof pins them again.  A prover that is dropped frees
+        them too (a finalizer that keeps the context alive until it has run)"""
+        if self._pinned:
+            self._pinned[2]()
+            self._pinned = None
+
+    def _host_heaps(self, nbytes):
+        """a uint8 view of at least nbytes of pinned host memory: the held allocation while it is large enough"""
+        if self._pinned and self._pinned[1] < nbytes:
+            self.release_host_memory()
+        if not self._pinned:
+            addr = self.ctx.alloc_host_pinned(nbytes)
+            self._pinned = (addr, nbytes, weakref.finalize(self, _free_pinned, self.ctx, addr))
+        return np.ctypeslib.as_array(C.cast(self._pinned[0], C.POINTER(C.c_uint8)), shape=(nbytes,))
 
     # ---- helpers
     def _to_device(self, a):
@@ -228,14 +268,22 @@ class GpuProver:
         return avail if cap is None else min(cap, avail)
 
     def choose_residency(self, est):
-        """"resident" if its estimate fits, else "streamed" if that fits, else ProvingError (nothing is allocated yet)"""
+        """"resident" if its estimate fits, else "streamed" if that fits, else "streamed_host" if its device estimate fits
+        and its node heaps fit host_memory_budget, else ProvingError (nothing is allocated yet)"""
         budget = self.memory_available()
         if est["resident"] <= budget:
             return "resident"
         if est["streamed"] <= budget:
             return "streamed"
-        raise ProvingError(f"the proof does not fit on the device: it needs about {_gib(est['resident'])} resident or "
-                           f"{_gib(est['streamed'])} streamed, and {_gib(budget)} is available")
+        host = self.host_memory_budget
+        if host is not None and est["streamed_host"] <= budget and est["host"] <= host:
+            return "streamed_host"
+        msg = (f"the proof does not fit on the device: it needs about {_gib(est['resident'])} resident or "
+               f"{_gib(est['streamed'])} streamed, and {_gib(budget)} is available")
+        if host is not None:
+            msg += (f"; with the Merkle node heaps in pinned host memory it needs about {_gib(est['streamed_host'])} on the "
+                    f"device and {_gib(est['host'])} of host memory, and {_gib(host)} of host memory is allowed")
+        raise ProvingError(msg)
 
     # ---- default_prove
     def prove(self, stark, options, witness, validate=False):
@@ -290,14 +338,23 @@ class GpuProver:
         beta = options.lde_blowup_factor
         log_b = beta.bit_length() - 1
         nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
-        residency = self.choose_residency(peak_bytes(n, beta, nbase, next_, fq, air.ce_blowup_factor, options.fri_folding_factor))
+        est = peak_bytes(n, beta, nbase, next_, fq, air.ce_blowup_factor, options.fri_folding_factor)
+        if self.pinned_bytes > (self.host_memory_budget or 0):
+            self.release_host_memory()          # heaps pinned under a larger budget are not held past a lower one
+        residency = self.choose_residency(est)
         self.last_residency = residency
         channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
         r = _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
                  beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
-                 timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate)
+                 timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate, host_heaps=None)
         lap("init_air")
-        return self._prove_resident(r) if residency == "resident" else self._prove_streamed(r)
+        if residency == "resident":
+            return self._prove_resident(r)
+        if residency == "streamed_host":
+            # tree t's node heap: beta local heaps of n digests (base, extension if any, composition)
+            r.host_heaps = self._host_heaps(est["host"])[:est["host"]].reshape(-1, beta, n, 32)
+            lap("pin_host_memory")
+        return self._prove_streamed(r)
 
     def _prove_resident(self, r):
         ctx, stark, trace, air, channel, lap = r.ctx, r.stark, r.trace, r.air, r.channel, r.lap
@@ -399,19 +456,31 @@ class GpuProver:
         return self._finish(r, fri_proof, queries)
 
     # ---- streamed residency: coefficients and tree nodes stay, coset blocks are recomputed
-    def _commit_blocks(self, polys, blk, field, ncols, log_n, log_b, offsets):
+    def _commit_blocks(self, polys, blk, field, ncols, log_n, log_b, offsets, host_heap=None):
         """Merkle commitment of the bit-reversed LDE of `polys`, one coset block at a time: block q is transformed into
         `blk` and hashed into its subtree of the node heap; the top log_b levels come from the block roots.
-        Returns (nodes, root)."""
+        Returns (nodes, root).  With host_heap ((beta, n, 32) bytes of pinned host memory), block q's subtree is its local
+        heap host_heap[q] and nodes is (top heap of 2 beta digests on the host, host_heap): the split layout of
+        include/ministark_host_nodes.h."""
         ctx, beta = self.ctx, 1 << log_b
-        nodes, roots = self._empty(beta << log_n, 4), self._empty(beta, 4)
+        if host_heap is None:
+            nodes, roots = self._empty(beta << log_n, 4), self._empty(beta, 4)
+        else:
+            nodes = self._empty(2 * beta, 4)
+            roots = nodes[beta:]
         for q, h in offsets:
             self._block(polys, blk, field, ncols, log_n, h)
-            ctx.merkle_commit_block(blk, field, log_n, log_b, q, ncols, nodes, roots[q])
+            if host_heap is None:
+                ctx.merkle_commit_block(blk, field, log_n, log_b, q, ncols, nodes, roots[q])
+            else:
+                ctx.merkle_commit_block_host(blk, field, log_n, ncols, host_heap[q], roots[q])
         if beta > 1:
             ctx.merkle_nodes(roots, nodes, beta)
         nodes[0].zero_()                        # the unused default digest (named by a walk over a 2-leaf tree)
-        return nodes, nodes[1].cpu().numpy().tobytes()
+        root = nodes[1].cpu().numpy().tobytes()
+        if host_heap is not None:
+            nodes = (nodes.cpu().numpy().view(np.uint8), host_heap)
+        return nodes, root
 
     def _block(self, polys, blk, field, ncols, log_n, h):
         """coset block with offset h of the bit-reversed LDE of every column of `polys`, into `blk`.  Its NTT plan is
@@ -432,7 +501,15 @@ class GpuProver:
             return hashlib.sha256(b"".join((int(w) * _RINV % P).to_bytes(8, "little") for w in row)).digest()
 
         digests = [leaf(row) for row in rows[k:]]
-        path_nodes = [d.tobytes() for d in self.ctx.gather_rows_rowmajor(nodes, 4, N, path)] if path else []
+        if isinstance(nodes, tuple):            # split heap: the top heap, then each block's local heap
+            top, blocks = nodes
+            self.ctx.sync()                     # the last blocks' copies to host memory
+            path_nodes = []
+            for i in path:
+                b, j = heap_location(i, log_b)
+                path_nodes.append((top[j] if b is None else blocks[b, j]).tobytes())
+        else:
+            path_nodes = [d.tobytes() for d in self.ctx.gather_rows_rowmajor(nodes, 4, N, path)] if path else []
         return rows[:k], MerkleView(path_nodes, digests[:len(init)], digests[len(init):], N.bit_length() - 1)
 
     def _prove_streamed(self, r):
@@ -448,7 +525,8 @@ class GpuProver:
         del host_base                           # held no longer than `base`: see release_base_columns below
         base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
         ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
-        base_nodes, base_root = self._commit_blocks(base_polys, base_blk, FP, nbase, log_n, log_b, offsets)
+        heaps = r.host_heaps if r.host_heaps is not None else [None] * 3
+        base_nodes, base_root = self._commit_blocks(base_polys, base_blk, FP, nbase, log_n, log_b, offsets, heaps[0])
         channel.commit_base_trace(base_root)
         lap("base_trace_commitment")
         challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
@@ -465,7 +543,7 @@ class GpuProver:
             ctx.ntt_batch_to(self._to_device(ext), ext_polys, fq, log_n, next_, inverse=True)
             del ext
             ext_blk = self._empty(next_, n * fq)
-            ext_nodes, ext_root = self._commit_blocks(ext_polys, ext_blk, fq, next_, log_n, log_b, offsets)
+            ext_nodes, ext_root = self._commit_blocks(ext_polys, ext_blk, fq, next_, log_n, log_b, offsets, heaps[1])
             channel.commit_extension_trace(ext_root)
         lap("extension_trace_commitment")
         self._check(r, challenges, hints, check)
@@ -494,12 +572,16 @@ class GpuProver:
 
         # ---- composition trace: the bit-reversed ce-domain column -> coefficients -> ce_blowup columns
         ctx.bit_reverse(comp_evals, fq, log_ce)
+        if r.host_heaps is not None:
+            # the size-M transform's temporary (as large as the column: 12 GiB at 2^25 rows) is the context's own
+            # allocation and cannot reuse blocks torch's allocator keeps cached from the trace and extension columns
+            torch.cuda.empty_cache()
         ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
         comp_polys = self._composition_columns(r, comp_evals)
         del comp_evals                          # (when ce_blowup == 1, comp_polys is a view of it and keeps it)
         ctx.set_option("drop_scratch", 1)       # the size-M transform's temporary: as large as the column itself
         comp_blk = self._empty(ce_blowup, n * fq)
-        comp_nodes, comp_root = self._commit_blocks(comp_polys, comp_blk, fq, ce_blowup, log_n, log_b, offsets)
+        comp_nodes, comp_root = self._commit_blocks(comp_polys, comp_blk, fq, ce_blowup, log_n, log_b, offsets, heaps[-1])
         channel.commit_composition_trace(comp_root)
         lap("composition_trace_commitment")
 

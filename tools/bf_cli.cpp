@@ -1,10 +1,11 @@
 // bf_cli.cpp — the brainfuck prover and verifier on the command line (examples/brainfuck/main.rs), over the C++ host layer:
 //
-//   ministark_bf prove SRC --dst FILE [--input STR] [--memory-budget GIB] [--device K]
+//   ministark_bf prove SRC --dst FILE [--input STR] [--memory-budget GIB] [--host-memory GIB] [--device K]
 //   ministark_bf verify SRC --proof FILE [--input STR] --output STR
 //
 // prove builds the execution trace on the device (bf::simulate_device), proves it with mshost::GpuProver in whichever
-// residency fits (resident, else streamed, else it refuses) and writes the reference's (claim, proof).serialize_compressed:
+// residency fits (resident, else streamed, else, with --host-memory, streamed with the Merkle node heaps in that much
+// pinned host memory, else it refuses) and writes the reference's (claim, proof).serialize_compressed:
 // claim_bytes(source, input, output) followed by the proof bytes.  verify needs no GPU: it parses the claim, checks it
 // against the arguments and runs mshost::verify at the reference's 96-bit security level.  Either exits non-zero with a
 // message where the reference panics.
@@ -30,7 +31,7 @@ struct Failure : std::runtime_error {
 
 int usage() {
     fprintf(stderr,
-            "usage: ministark_bf prove SRC --dst FILE [--input STR] [--memory-budget GIB] [--device K]\n"
+            "usage: ministark_bf prove SRC --dst FILE [--input STR] [--memory-budget GIB] [--host-memory GIB] [--device K]\n"
             "       ministark_bf verify SRC --proof FILE [--input STR] --output STR\n");
     return 2;
 }
@@ -45,12 +46,14 @@ double seconds_since(std::chrono::steady_clock::time_point t0) {
     return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
-int run_prove(const std::string &src_path, const std::string &dst, const std::string &input_str, double budget_gib, int device) {
+int run_prove(const std::string &src_path, const std::string &dst, const std::string &input_str, double budget_gib, double host_gib,
+              int device) {
     const Bytes src_bytes = read_file(src_path);
     const std::string source(src_bytes.begin(), src_bytes.end());
     const Bytes input(input_str.begin(), input_str.end());
     GpuProver prover(device);
     if (budget_gib > 0) prover.memory_budget = (u64)(budget_gib * (double)((u64)1 << 30));
+    if (host_gib > 0) prover.host_memory_budget = (u64)(host_gib * (double)((u64)1 << 30));
 
     const u64 free_before = prover.free_memory();
     auto t0 = std::chrono::steady_clock::now();
@@ -69,6 +72,9 @@ int run_prove(const std::string &src_path, const std::string &dst, const std::st
                                      });
     printf("Proof generated in: %.3fs\n", seconds_since(t0));
     printf("Residency: %s\n", prover.last_residency.c_str());
+    if (prover.pinned_bytes())
+        printf("Pinned host memory: %llu bytes (%s), pinned in %.3fs\n", (unsigned long long)prover.pinned_bytes(),
+               gib(prover.pinned_bytes()).c_str(), prover.last_pin_seconds);
     if (free_before != SIZE_MAX) {
         printf("Free device memory before the trace: %llu bytes (%s)\n", (unsigned long long)free_before, gib(free_before).c_str());
         printf("Lowest free device memory between phases: %llu bytes (%s)\n", (unsigned long long)prover.lowest_free_bytes,
@@ -124,7 +130,7 @@ int main(int argc, char **argv) {
     const std::string cmd = argv[1], src = argv[2];
     std::string dst, proof, input, output;
     bool has_output = false;
-    double budget = 0;
+    double budget = 0, host_memory = 0;
     int device = 0;
     for (int i = 3; i < argc; i++) {
         const std::string a = argv[i];
@@ -138,11 +144,15 @@ int main(int argc, char **argv) {
             char *end = nullptr;
             budget = strtod(v.c_str(), &end);
             if (*end || !(budget > 0)) return usage();
+        } else if (a == "--host-memory") {
+            char *end = nullptr;
+            host_memory = strtod(v.c_str(), &end);
+            if (*end || !(host_memory > 0)) return usage();
         } else if (a == "--device") device = atoi(v.c_str());
         else return usage();
     }
     try {
-        if (cmd == "prove" && !dst.empty()) return run_prove(src, dst, input, budget, device);
+        if (cmd == "prove" && !dst.empty()) return run_prove(src, dst, input, budget, host_memory, device);
         if (cmd == "verify" && !proof.empty() && has_output) return run_verify(src, proof, input, output);
     } catch (const std::exception &e) {
         fprintf(stderr, "ministark_bf %s: %s\n", cmd.c_str(), e.what());
