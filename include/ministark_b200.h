@@ -73,7 +73,9 @@ const char *ms_version(void);
  * TMA pipeline for the 256 x 16 tile NTT passes (default 1), "ntt_tma_groups" 2|3 consumer groups per CTA,
  * "ntt_tma_stages" 3..8 cap on its shared-memory ring; "drop_plans" (any value) frees this context's cached NTT plans and
  * their twiddle / scale tables (hundreds of MiB for 2^24-point LDE plans; rebuilt on demand); "drop_scratch" (any value)
- * frees its scratch arenas (e.g. the temporary of a large single-column transform; regrown on demand). */
+ * frees its scratch arenas (e.g. the temporary of a large single-column transform; regrown on demand).  Test switches:
+ * "ntt_table_words" (per context, -1 = built-in limits) caps in words each full twiddle / scale table of new plans and
+ * drops the cached plans; "ntt_wide_index" 0|1 makes the tile passes use their 64-bit-offset instantiations at every size. */
 int ms_set_option(ms_ctx *ctx, const char *name, int64_t value);
 /* number of kernels this context has launched so far (bench.py "gpu_launches") */
 uint64_t ms_launch_count(ms_ctx *ctx);

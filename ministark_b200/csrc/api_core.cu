@@ -225,10 +225,20 @@ int ms_ctx_sync(ms_ctx *c) {
     return ms::host_nodes_drain(c, false);     // node heaps still crossing to host memory
 }
 
-// tuning / A-B switches (process-wide): "ntt_tma" 0|1, "ntt_tma_groups" 2|3, "ntt_tma_stages" 3..8
+// tuning / A-B switches (process-wide): "ntt_tma" 0|1, "ntt_tma_groups" 2|3, "ntt_tma_stages" 3..8, "ntt_wide_index" 0|1;
+// per context: "ntt_table_words"
 int ms_set_option(ms_ctx *c, const char *name, int64_t value) {
     if (!name) return MS_ERR_INVALID;
     if (!strcmp(name, "ntt_tma")) { msntt::tma_configure(value ? 1 : 0, 0, 0); return MS_OK; }
+    if (!strcmp(name, "ntt_wide_index")) { msntt::wide_index_configure(value ? 1 : 0); return MS_OK; }
+    if (!strcmp(name, "ntt_table_words")) {   // cap on the full tables of this context's plans; cached plans are dropped
+        if (!c) return MS_ERR_INVALID;
+        if (value < -1) return fail(c, MS_ERR_INVALID, "ntt_table_words must be -1 (built-in limits) or >= 0");
+        cudaSetDevice(c->device);
+        ms::ntt_drop_plans(c);
+        c->ntt_table_words = value;
+        return MS_OK;
+    }
     if (!strcmp(name, "ntt_tma_groups")) {
         if (value != 2 && value != 3) return fail(c, MS_ERR_INVALID, "ntt_tma_groups must be 2 or 3");
         msntt::tma_configure(-1, (int)value, 0);

@@ -215,7 +215,11 @@ int ntt_get_plan(ms_ctx *c, const NttJob &job, std::shared_ptr<NttPlanDev> *out)
             P->big.push_back(d);
             return d;
         };
-        const size_t kOuterMax = (size_t)64 << 20, kPreMax = (size_t)256 << 20;  // words (512 MiB / 2 GiB)
+        size_t kOuterMax = (size_t)64 << 20, kPreMax = (size_t)256 << 20;  // words (512 MiB / 2 GiB)
+        if (c->ntt_table_words >= 0) {  // "ntt_table_words": a lower cap; 0 leaves every factor to the progressions
+            kOuterMax = std::min(kOuterMax, (size_t)c->ntt_table_words);
+            kPreMax = std::min(kPreMax, (size_t)c->ntt_table_words);
+        }
         for (size_t k = 0; k < P->passes.size(); k++) {
             PassParams &p = P->passes[k];
             if (p.has_outer) {

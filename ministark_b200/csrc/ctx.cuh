@@ -47,6 +47,7 @@ struct ms_ctx {
     ms::Scratch scratch[4];            // grow-only device arenas (0: ntt tmp, 1: staging in, 2: staging out, 3: misc)
     ms::u64 *t4096[2] = {nullptr, nullptr};  // omega_4096^e forward / inverse
     std::map<std::tuple<int, unsigned, int, uint64_t, unsigned, int>, std::shared_ptr<ms::NttPlanDev>> plans;
+    int64_t ntt_table_words = -1;      // "ntt_table_words": cap in words on each full table a new plan builds (-1: built-in limits)
     std::deque<ms::PtrTable> ptr_tables;       // cached device copies of LDE scatter pointer tables (deque: stable addresses)
     std::map<unsigned, ms::u64 *> tw_tables;   // log_n -> two-level g_n^e table (4096 + n/4096 words), ntt_plan_tables
     // ms_merkle_commit_block_sha256_host: block heaps are built in node_stage[k] and copied to pinned host memory on

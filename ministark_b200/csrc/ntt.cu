@@ -393,11 +393,14 @@ static void launch_t(const PassParams &p, const Tables &t, bool inverse, const u
     }
 }
 
+static bool g_wide_index = false;
+void wide_index_configure(int enabled) { g_wide_index = enabled != 0; }
+
 void launch_pass(const PassParams &p, const Tables &t, bool inverse, const u64 *in, u64 *out, unsigned ntiles,
                  unsigned nbatch, cudaStream_t stream) {
     // the shapes large transforms are made of get log2(W) fixed at compile time
     // ... provided every word offset inside a column (and inside the twiddle / scale tables) fits in 32 bits
-    const bool small = ((p.n_mask + 1) * (u64)p.estride) <= (1ull << 31);
+    const bool small = !g_wide_index && ((p.n_mask + 1) * (u64)p.estride) <= (1ull << 31);
     if (!small) goto generic;
     if (p.log_r == 8 && p.log_w == 4) return launch_t<8, 4>(p, t, inverse, in, out, ntiles, nbatch, stream);
     if (p.log_r == 7 && p.log_w == 5) return launch_t<7, 5>(p, t, inverse, in, out, ntiles, nbatch, stream);

@@ -94,6 +94,9 @@ void launch_naive(const u64 *in, u64 in_stride_words, u64 *out, u64 out_stride_w
 bool launch_pass_tma(const PassParams &p, const Tables &t, bool inverse, const u64 *in, u64 *out, unsigned ntiles,
                      unsigned ncols, cudaStream_t stream);
 void tma_configure(int enabled, int groups, int max_stages);
+// wide_index_configure(1): launch_pass uses the 64-bit-offset instantiations (LW = -1) at every size instead of the
+// compile-time (8,4) / (7,5) / (6,6) tile shapes, so that path can be compared with the oracle at small sizes
+void wide_index_configure(int enabled);
 // table builders (device kernels): dst[i] = lookup2(lo, hi, hi_len, i) and the outer-twiddle table
 void build_pow_table(u64 *dst, u64 count, const u64 *lo, const u64 *hi, u32 hi_len, cudaStream_t stream);
 void build_outer_table(u64 *dst, u64 R, u64 S, u64 mult, u64 n_mask, const u64 *lo, const u64 *hi, u32 hi_len,

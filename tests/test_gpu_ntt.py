@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import ministark_b200 as ms
+from tests_helpers_ntt import edge_column, structured_columns
 
 pytestmark = pytest.mark.gpu
 
@@ -17,23 +18,13 @@ def ctx():
     return ms.Context(0)
 
 
-def _edge_column(n, lanes, rng):
-    """random words seasoned with the values that break lazy/modular arithmetic"""
-    P = ms.P
-    edge = np.array([0, 1, P - 1, P - 2, 2**32 - 1, 2**32, 2**32 + 1, 0xFFFFFFFF00000000, 2**63, P - 2**32], dtype=np.uint64)
-    v = rng.integers(0, P, size=n * lanes, dtype=np.uint64)
-    k = min(len(edge), v.size)
-    v[rng.choice(v.size, size=k, replace=False)] = edge[:k]
-    return v
-
-
 @pytest.mark.parametrize("log_n", list(range(0, 19)))
 @pytest.mark.parametrize("coset", [False, True])
 def test_fft_ifft_fp_all_sizes(ctx, orc, log_n, coset):
     rng = np.random.default_rng(log_n * 2 + coset)
     n = 1 << log_n
     offset = orc.generator() if coset else orc.ONE
-    col = _edge_column(n, 1, rng)
+    col = edge_column(n, 1, rng)
     # GpuFft::encode / execute on a host slice (gpu/tests/shaders.rs:17-40)
     got = col.copy()
     fft = ms.GpuFft(ms.Domain(log_n, offset), ms.FP, ctx)
@@ -56,7 +47,7 @@ def test_fft_fq3(ctx, orc, log_n, coset):
     # gpu/tests/shaders.rs:43-66: Fq3 coefficients, Fp twiddles
     rng = np.random.default_rng(100 + log_n)
     offset = orc.generator() if coset else orc.ONE
-    col = _edge_column(1 << log_n, 3, rng)
+    col = edge_column(1 << log_n, 3, rng)
     got = col.copy()
     fft = ms.GpuFft(ms.Domain(log_n, offset), ms.FQ3, ctx)
     fft.encode(got)
@@ -215,29 +206,13 @@ def test_lazy_primitives_all_edge_pairs(ctx):
         assert int(out[4, i]) == x * yc * RINV % P, ("mul", hex(x), hex(y))
 
 
-def _structured_columns(n, rng):
-    """columns a real execution trace has: constants, 0/1 flags, counters, a handful of repeated values such as the
-    Montgomery words of 1/2 = 2^63 and 1/4 = 2^62 (their pairwise sums hit 2^64 exactly), runs, alternations"""
-    R, P = 2**64, ms.P
-    mont = lambda v: np.array([int(x) * R % P for x in v], dtype=np.uint64)
-    inv = [0] + [pow(v, -1, P) for v in range(1, 9)]
-    cols = [
-        np.zeros(n, dtype=np.uint64), np.full(n, ms.ONE, dtype=np.uint64), np.full(n, 2**63, dtype=np.uint64), np.full(n, P - 1, dtype=np.uint64),
-        mont(np.arange(n) % 2), mont(np.arange(n)), mont([inv[int(k)] for k in rng.integers(0, 5, size=n)]),
-        mont([inv[(i // 3) % 9] for i in range(n)]), np.where(np.arange(n) % 2 == 0, np.uint64(2**63), np.uint64(2**62)),
-        np.where(np.arange(n) < n // 2, np.uint64(2**63), np.uint64(0)), mont([P - 1 - (i % 4) for i in range(n)]),
-        np.where(rng.integers(0, 2, size=n) == 0, np.uint64(2**63), np.uint64(P - 2**63)),
-    ]
-    return np.stack(cols)
-
-
 @pytest.mark.parametrize("log_n", list(range(1, 17)))
 def test_structured_columns_all_transforms(ctx, orc, log_n):
     """forward / inverse, subgroup / coset NTT and the coset LDE on structured columns (the brainfuck MemValInv column —
     values 0, 1, 1/2, 1/3, 1/4 — exposed a spurious second carry in add_ll when two words sum to exactly 2^64)"""
     rng = np.random.default_rng(log_n)
     n = 1 << log_n
-    cols = _structured_columns(n, rng)
+    cols = structured_columns(n, rng)
     k = cols.shape[0]
     for inverse in (False, True):
         for offset in (orc.ONE, orc.generator()):
