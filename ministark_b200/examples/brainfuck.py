@@ -600,6 +600,8 @@ class BrainfuckAirConfig(AirConfig):
         ch = [tuple(c) for c in challenges]
 
         def io_terminal(symbols, challenge):
+            if trace_len < len(symbols):        # a verifier handed a forged trace length: the offset would be negative
+                raise ValueError(f"trace length {trace_len} is shorter than the {len(symbols)} input / output symbols")
             acc = (0, 0, 0)
             for s in symbols:
                 acc = E.q_add(E.q_mul(challenge, acc), (s, 0, 0))

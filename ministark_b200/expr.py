@@ -49,6 +49,8 @@ def q_mul(a, b):
 
 
 def q_pow(a, e):
+    if e < 0:
+        raise ValueError(f"negative exponent {e}")
     r = (1, 0, 0)
     while e:
         if e & 1:
@@ -147,6 +149,59 @@ def Periodic(coeffs, interval_size):
     if n == 0 or n & (n - 1) or m & (m - 1) or n > m:
         raise ValueError("periodic column: lengths must be powers of two with len(coeffs) <= interval_size")
     return Expr("periodic", coeffs, m)
+
+
+def evaluate_at(expr, x, trace=None, challenges=(), hints=(), ccoefs=(), trace_len=None):
+    """the value of `expr` at ONE point, on the host: Expr::graph_eval with the leaves of the verifier's out-of-domain
+    check (src/verifier.rs:207-229).  x: the point; trace: {(column, offset): value}; challenges / hints / ccoefs: the
+    values of Challenge(i) / Hint(i) / CompositionCoeff(i); Periodic(coeffs, interval) is its polynomial at
+    x^(trace_len / interval).  Values are canonical ints or 3-tuples; the result is a 3-tuple.  A zero denominator raises
+    ZeroDivisionError."""
+    post, seen, stack = [], set(), [(expr, False)]
+    while stack:                       # iterative post-order (DAGs can be deep)
+        node, done = stack.pop()
+        if done:
+            post.append(node)
+            continue
+        if id(node) in seen:
+            continue
+        seen.add(id(node))
+        stack.append((node, True))
+        stack.extend((a, False) for a in node.args if isinstance(a, Expr) and id(a) not in seen)
+    x = _q(x)
+    val = {}
+    for nd in post:
+        k, a = nd.kind, nd.args
+        if k == "x":
+            v = x
+        elif k == "const":
+            v = a[0]
+        elif k in _SYMBOLIC:
+            v = _q({"chal": challenges, "hint": hints, "ccoef": ccoefs}[k][a[0]])
+        elif k == "trace":
+            v = _q(trace[(a[0], a[1])])
+        elif k == "periodic":
+            y = q_pow(x, trace_len // a[1])
+            v = (0, 0, 0)
+            for c in reversed(a[0]):
+                v = q_add(q_mul(v, y), _q(c))
+        elif k == "neg":
+            v = q_neg(val[id(a[0])])
+        elif k == "add":
+            v = q_add(val[id(a[0])], val[id(a[1])])
+        elif k == "mul":
+            v = q_mul(val[id(a[0])], val[id(a[1])])
+        elif k in ("div", "inv"):
+            d = val[id(a[-1])]
+            if not any(d):
+                raise ZeroDivisionError(f"zero denominator in a {k} node")
+            v = q_inv(d) if k == "inv" else q_mul(val[id(a[0])], q_inv(d))
+        elif k == "pow":
+            v = q_pow(val[id(a[0])], a[1])
+        else:
+            raise ValueError(f"unsupported node {k}")
+        val[id(nd)] = v
+    return val[id(expr)]
 
 
 class Program:

@@ -31,6 +31,7 @@ import torch
 from . import FP, FQ3, GENERATOR as GEN_MONT, ONE, Context
 from . import deep
 from . import expr as E
+from . import verifier
 from .air import Air
 from .channel import ProverChannel, PublicCoin, serialize_element
 from .cosets import block_program, coset_offsets, heap_location, merkle_walk
@@ -118,6 +119,15 @@ class Stark:
         on first use and reused, like the reference's process-global Planner.  validate=True: check the trace against
         the AIR before the composition polynomial is computed (validate_constraints)."""
         return GpuProver.shared(device).prove(self, options, witness, validate=validate)
+
+    def verify(self, proof, required_security_bits):
+        """Stark::verify (src/stark.rs:78-84): default_verify of `proof` — a Proof, or its bytes (Proof.from_bytes with
+        this claim's field) — against this claim, on the host (ministark_b200/verifier.py).  Returns the
+        VerifierChannelArtifacts; raises verifier.VerificationError, or proof.ProofFormatError for bytes that are not a
+        proof."""
+        if isinstance(proof, (bytes, bytearray, memoryview)):
+            proof = Proof.from_bytes(proof, self.AirConfig.FQ_IS_FP)
+        return verifier.verify(self, proof, required_security_bits)
 
     def validate_constraints(self, air, challenges, hints, base_trace, extension_trace, ctx):
         """Stark::validate_constraints (src/stark.rs:65-75), called by `prove(..., validate=True)` right after the
