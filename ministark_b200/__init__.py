@@ -324,6 +324,21 @@ class Context:
                                                first_row.ctypes.data, fail_count.ctypes.data))
         return first_row, fail_count
 
+    def extension_columns(self, program, out, log_n, cols, cols_are_fq, fq_field, init, inclusive):
+        """the declared extension columns of an AIR (include/ministark_extension.h): column k is x_0 = init[k],
+        x_(i+1) = x_i * mul_k(i) + add_k(i) over the trace domain 2^log_n, with mul_k / add_k slots 2k / 2k + 1 of `program`
+        (expr.compile_extension_program, bound); row i holds x_(i+1) where inclusive[k], else x_i.  `cols`: natural-order
+        device columns, then the program's periodic tables; init: (K, fq_field) Montgomery words; out: a device matrix of K
+        columns of 2^log_n Fq elements."""
+        k = len(cols)
+        ptrs = (C.c_void_p * max(k, 1))(*[_ptr(c) for c in cols])
+        isq = (C.c_int * max(k, 1))(*[int(bool(q)) for q in cols_are_fq])
+        ini = np.ascontiguousarray(init, dtype=np.uint64).reshape(-1)
+        inc = (C.c_int * max(len(inclusive), 1))(*[int(bool(v)) for v in inclusive])
+        self._ck(self.lib.ms_extension_columns(self.h, program.code.ctypes.data, len(program), program.consts.ctypes.data,
+                                               program.consts.shape[0], ptrs, isq, k, fq_field, log_n, len(inclusive),
+                                               ini.ctypes.data, inc, _ptr(out)))
+
     def poly_eval(self, coeffs, field, n, ncols, points, col_stride=None):
         """horner_evaluate of every column at every point (get_ood_evals, src/composer.rs:43-86).
         points: (k, 3) Montgomery words; returns (ncols, k, 3) numpy uint64."""

@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("MS_LIB_PATH") or os.path.join(_HERE, "libministark_b2
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h")
 STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
+EXTENSION_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_extension.h")
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
@@ -80,6 +81,11 @@ _CHECK_SIGS = {
     "ms_check_constraints": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ci, ui, ui, vp, vp]),
 }
 
+# include/ministark_extension.h: extension columns declared by the AIR (air.RunningColumn), built on the device
+_EXTENSION_SIGS = {
+    "ms_extension_columns": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ci, ui, ui, vp, vp, vp]),
+}
+
 # include/ministark_bf.h: the execution trace of examples/brainfuck (VM on the host, tables on the device)
 _BF_SIGS = {
     "ms_bf_run": (ci, [vp, sz, vp, sz, u64, vp, vp, vp]),
@@ -127,6 +133,7 @@ def load():
         bind(lib, _SIGS)
         bind(lib, _STREAM_SIGS)
         bind(lib, _CHECK_SIGS)
+        bind(lib, _EXTENSION_SIGS)
         bind(lib, _BF_SIGS)
         bind(lib, _DEVICE_SIGS)
         bind(lib, _HOST_NODES_SIGS)

@@ -10,6 +10,9 @@ Trace(column, offset) | Periodic(coeffs, interval_size) plus, inside the
 composition constraint only, CompositionCoeff(i) — the verifier randomness that is substituted as
 constants once the channel has produced it (src/air.rs:96-101).
 
+Extension columns may be declared the same way (AirConfig.extension_columns, RunningColumn): the prover then builds them
+on the device from the base trace instead of calling a host builder.
+
 This module is pure bookkeeping (a few hundred DAG nodes): no field data is touched here.
 """
 from dataclasses import dataclass
@@ -142,6 +145,32 @@ def _leaves(expr, kind):
     return out
 
 
+MAX_DECLARED_COLUMNS = 8                         # csrc/extension.cu builds at most this many columns in one pass
+
+
+@dataclass(frozen=True)
+class RunningColumn:
+    """One declared extension column: x_0 = init, x_(i+1) = x_i * mul(i) + add(i) over the trace domain, a running
+    product (add = 0), running evaluation (mul = a challenge) or running sum (mul = 1).  Row i holds x_i, or x_(i+1) when
+    `inclusive`.  Values are in Fq (Fq3, or Fp when FQ_IS_FP).
+
+    mul / add: Exprs (or field values) over Constant, Challenge, Hint, X, Periodic and Trace(c, offset) of a BASE column
+    c, any offset; the row index wraps mod n as in constraint evaluation on the trace domain, and X at row i is g_n^i.
+    Division is allowed, and a zero denominator gives 0 (the inverse of zero is zero), so a LogUp-style
+    add = m / (alpha - t) - 1 / (alpha - v) can be declared.  init: an Expr (or field value) over Constant, Challenge and
+    Hint only, evaluated on the host."""
+    init: object
+    mul: object = 1
+    add: object = 0
+    inclusive: bool = False
+
+
+def _as_expr(v):
+    if isinstance(v, E.Expr):
+        return v
+    return E.Constant(tuple(v)) if isinstance(v, (tuple, list)) else E.Constant(v)
+
+
 class AirConfig:
     """Subclass and override, as with the reference's trait (src/air.rs:26-48).  Field values handed to and
     returned by the hooks are canonical integers (Fp) or 3-tuples of canonical integers (Fq3)."""
@@ -160,6 +189,13 @@ class AirConfig:
     @staticmethod
     def domain_offset():
         return GENERATOR
+
+    @staticmethod
+    def extension_columns(trace_len):
+        """None (the trace builds its own extension columns), or one RunningColumn per extension column, in column
+        order: the prover then builds them on the device from the base trace whenever the trace brings no builder of its
+        own.  A declaration adds no constraint: the AIR's constraints must still enforce every declared column."""
+        return None
 
 
 class Air:
@@ -186,6 +222,44 @@ class Air:
         self.composition_constraint = total
         self.ce_blowup_factor = blowup_factor(total, trace_len)
         assert self.ce_blowup_factor <= options.lde_blowup_factor
+        hook = getattr(config, "extension_columns", None)
+        self.extension_declaration = self._declaration(hook(trace_len) if hook is not None else None)
+
+    def _declaration(self, decl):
+        """AirConfig.extension_columns checked against the AIR: RunningColumns with Expr fields, or ValueError"""
+        if decl is None:
+            return None
+        cfg = self.config
+        decl = list(decl)
+        if len(decl) != cfg.NUM_EXTENSION_COLUMNS:
+            raise ValueError(f"extension_columns declares {len(decl)} columns but NUM_EXTENSION_COLUMNS is "
+                             f"{cfg.NUM_EXTENSION_COLUMNS}")
+        if len(decl) > MAX_DECLARED_COLUMNS:
+            raise ValueError(f"extension_columns declares {len(decl)} columns; at most {MAX_DECLARED_COLUMNS} can be built")
+        nchal = self.num_challenges()
+        out = []
+        for k, col in enumerate(decl):
+            c = cfg.NUM_BASE_COLUMNS + k
+            if not isinstance(col, RunningColumn):
+                raise ValueError(f"extension column {c}: expected a RunningColumn, got {type(col).__name__}")
+            col = RunningColumn(_as_expr(col.init), _as_expr(col.mul), _as_expr(col.add), bool(col.inclusive))
+            for name in ("init", "mul", "add"):
+                e = getattr(col, name)
+                for kind in ("ccoef",) + (("trace", "x", "periodic") if name == "init" else ()):
+                    if _leaves(e, kind):
+                        what = {"ccoef": "a composition coefficient", "trace": "the trace", "x": "X",
+                                "periodic": "a periodic column"}[kind]
+                        raise ValueError(f"extension column {c}: {name} reads {what}")
+                for col_idx, off in sorted(_leaves(e, "trace")):
+                    if not 0 <= col_idx < cfg.NUM_BASE_COLUMNS:
+                        raise ValueError(f"extension column {c}: {name} reads Trace({col_idx}, {off}), which is not a base "
+                                         f"column (0..{cfg.NUM_BASE_COLUMNS - 1})")
+                for (i,) in sorted(_leaves(e, "chal")):
+                    if i >= nchal:
+                        raise ValueError(f"extension column {c}: {name} reads Challenge({i}), but the constraints make the "
+                                         f"channel draw {nchal} challenges")
+            out.append(col)
+        return out
 
     def lde_blowup_factor(self):
         return self.options.lde_blowup_factor
@@ -220,6 +294,16 @@ class Air:
             self._check_program = E.compile_check_program(self.constraints, cfg.NUM_BASE_COLUMNS, self.log_n,
                                                           cfg.NUM_BASE_COLUMNS + cfg.NUM_EXTENSION_COLUMNS)
         return self._check_program
+
+    def extension_program(self):
+        """the declared extension columns' row maps as one evaluator program (csrc/extension.cu; challenges and hints are
+        bound per proof), or None without a declaration"""
+        if getattr(self, "_extension_program", None) is None and self.extension_declaration:
+            d = self.extension_declaration
+            self._extension_program = E.compile_extension_program([c.mul for c in d], [c.add for c in d],
+                                                                  self.config.NUM_BASE_COLUMNS, self.log_n,
+                                                                  self.config.NUM_BASE_COLUMNS)
+        return getattr(self, "_extension_program", None)
 
     # the three walks below depend on the constraints only: done once per Air (the provers copy a cached Air per proof,
     # and each walk of the brainfuck AIR costs ~0.5 ms of a 10 ms proof)

@@ -51,136 +51,20 @@ __global__ void __launch_bounds__(128) eval_kernel(const EvalParams p) {
     const u64 i = (p.trace_bitrev && lm) ? (__brevll(t) >> (64 - lm)) : t;   // evaluation point index
     const bool fq3 = p.fq_words == 3;
     u64 r[kMaxRegs][3];
-
-    for (u32 pc = 0; pc < p.nprog; pc++) {
-        const uint4 ins = __ldg(p.prog + pc);
-        const u32 op = ins.x & 0xff;
-        const bool qa = ((ins.x >> 8) & 1) && fq3, qb = ((ins.x >> 9) & 1) && fq3;
-        const u32 d = ins.y;
-        switch (op) {
-            case OP_X: {
-                u64 w = p.tw_lo[i & 4095];
-                if (p.hi_len > 1) w = gl::mul(p.tw_hi[i >> 12], w);
-                r[d][0] = gl::mul(w, p.offset);
-                break;
-            }
-            case OP_CONST: {
-                const u64 *k = p.consts + 3 * (u64)ins.z;
-                r[d][0] = k[0];
-                if (qa) { r[d][1] = k[1]; r[d][2] = k[2]; }
-                break;
-            }
-            case OP_TRACE: {
-                u64 pos = (i + (u64)ins.w) & (M - 1);
-                if (p.trace_bitrev && lm) pos = __brevll(pos) >> (64 - lm);
-                const u64 *col = p.col_ptr[ins.z];
-                if ((ins.x >> 8) & 1) {  // Fq column
-                    const u64 *c = col + pos * p.fq_words;
-                    r[d][0] = c[0];
-                    if (fq3) { r[d][1] = c[1]; r[d][2] = c[2]; }
-                } else {
-                    r[d][0] = col[pos];
-                }
-                break;
-            }
-            case OP_NEG: {
-                const u64 a0 = r[ins.z][0];
-                if (qa) {
-                    const u64 a1 = r[ins.z][1], a2 = r[ins.z][2];
-                    r[d][1] = gl::neg(a1);
-                    r[d][2] = gl::neg(a2);
-                }
-                r[d][0] = gl::neg(a0);
-                break;
-            }
-            case OP_ADD: {
-                const u64 a0 = r[ins.z][0], b0 = r[ins.w][0];
-                if (qa || qb) {
-                    const u64 a1 = qa ? r[ins.z][1] : 0, a2 = qa ? r[ins.z][2] : 0;
-                    const u64 b1 = qb ? r[ins.w][1] : 0, b2 = qb ? r[ins.w][2] : 0;
-                    r[d][1] = gl::add(a1, b1);
-                    r[d][2] = gl::add(a2, b2);
-                }
-                r[d][0] = gl::add(a0, b0);
-                break;
-            }
-            case OP_SUB: {
-                const u64 a0 = r[ins.z][0], b0 = r[ins.w][0];
-                if (qa || qb) {
-                    const u64 a1 = qa ? r[ins.z][1] : 0, a2 = qa ? r[ins.z][2] : 0;
-                    const u64 b1 = qb ? r[ins.w][1] : 0, b2 = qb ? r[ins.w][2] : 0;
-                    r[d][1] = gl::sub(a1, b1);
-                    r[d][2] = gl::sub(a2, b2);
-                }
-                r[d][0] = gl::sub(a0, b0);
-                break;
-            }
-            case OP_PERIODIC: {
-                // periodic column (src/constraints.rs:107-146, src/eval_cpu.rs:234-256): a table of 2^ins.w evaluations
-                // over the coset of size interval * lde_step, repeated along the ce domain; natural order
-                const u64 pos = i & ((1ull << ins.w) - 1);
-                const u64 *col = p.col_ptr[ins.z];
-                if ((ins.x >> 8) & 1) {
-                    const u64 *c = col + pos * p.fq_words;
-                    r[d][0] = c[0];
-                    if (fq3) { r[d][1] = c[1]; r[d][2] = c[2]; }
-                } else {
-                    r[d][0] = col[pos];
-                }
-                break;
-            }
-            case OP_MUL: {
-                if (!qa && !qb) {
-                    r[d][0] = gl::mul(r[ins.z][0], r[ins.w][0]);
-                } else if (qa && qb) {
-                    const Fq3 a{r[ins.z][0], r[ins.z][1], r[ins.z][2]}, b{r[ins.w][0], r[ins.w][1], r[ins.w][2]};
-                    const Fq3 c = gl::mul(a, b);
-                    r[d][0] = c.c0; r[d][1] = c.c1; r[d][2] = c.c2;
-                } else {
-                    const u32 q = qa ? ins.z : ins.w, s = qa ? ins.w : ins.z;
-                    const Fq3 a{r[q][0], r[q][1], r[q][2]};
-                    const Fq3 c = gl::mul(a, r[s][0]);
-                    r[d][0] = c.c0; r[d][1] = c.c1; r[d][2] = c.c2;
-                }
-                break;
-            }
-            case OP_INV: {
-                if (qa) {
-                    const Fq3 c = gl::inv(Fq3{r[ins.z][0], r[ins.z][1], r[ins.z][2]});
-                    r[d][0] = c.c0; r[d][1] = c.c1; r[d][2] = c.c2;
-                } else {
-                    r[d][0] = gl::inv(r[ins.z][0]);
-                }
-                break;
-            }
-            case OP_POW: {
-                if (qa) {
-                    const Fq3 c = gl::pow(Fq3{r[ins.z][0], r[ins.z][1], r[ins.z][2]}, (u64)ins.w);
-                    r[d][0] = c.c0; r[d][1] = c.c1; r[d][2] = c.c2;
-                } else {
-                    r[d][0] = gl::pow(r[ins.z][0], (u64)ins.w);
-                }
-                break;
-            }
-            case OP_STORE: {
-                u64 *o = p.out + (p.out_bitrev ? t : i) * p.fq_words;
-                o[0] = r[ins.z][0];
-                if (fq3) {
-                    o[1] = qa ? r[ins.z][1] : 0;
-                    o[2] = qa ? r[ins.z][2] : 0;
-                }
-                break;
-            }
-            default: break;
+    eval_point(p, M, i, r, [&](u32, const u64 *v, bool qa) {
+        u64 *o = p.out + (p.out_bitrev ? t : i) * p.fq_words;
+        o[0] = v[0];
+        if (fq3) {
+            o[1] = qa ? v[1] : 0;
+            o[2] = qa ? v[2] : 0;
         }
-    }
+    });
 }
 
 int validate_program(ms_ctx *c, const char *who, const uint32_t *program, unsigned nprog, unsigned nconsts,
-                     const std::vector<int> &col_is_q, unsigned log_m, unsigned nconstraints) {
+                     const std::vector<int> &col_is_q, unsigned log_m, unsigned nconstraints, unsigned nout) {
     const bool checked = nconstraints > 0;
-    std::vector<char> defined(kMaxRegs, 0);
-    bool stored = false;
+    std::vector<char> defined(kMaxRegs, 0), stored(checked ? 0 : nout, 0);
     for (unsigned k = 0; k < nprog; k++) {
         const uint32_t *ins = program + 4 * k;
         const uint32_t op = ins[0] & 0xff;
@@ -195,6 +79,8 @@ int validate_program(ms_ctx *c, const char *who, const uint32_t *program, unsign
             if (col_is_q[ins[2]] != is_q) return fail(c, MS_ERR_INVALID, "%s: column %u has the wrong field", who, ins[2]);
             if (op == OP_PERIODIC && ins[3] > log_m) return fail(c, MS_ERR_INVALID, "%s: periodic table longer than the domain", who);
         }
+        if (op == OP_STORE && ins[1] >= nout)
+            return fail(c, MS_ERR_INVALID, "%s: instruction %u stores to slot %u of %u", who, k, ins[1], nout);
         if (op == OP_CHECK && ins[3] >= nconstraints)
             return fail(c, MS_ERR_INVALID, "%s: instruction %u checks constraint %u of %u", who, k, ins[3], nconstraints);
         const bool unary = op == OP_NEG || op == OP_INV || op == OP_POW || op == OP_STORE || op == OP_CHECK;
@@ -207,10 +93,14 @@ int validate_program(ms_ctx *c, const char *who, const uint32_t *program, unsign
             if (ins[3] >= (uint32_t)kMaxRegs || !defined[ins[3]])
                 return fail(c, MS_ERR_INVALID, "%s: instruction %u reads register %u before it is written", who, k, ins[3]);
         }
-        if (op == OP_STORE) stored = true;
+        if (op == OP_STORE) stored[ins[1]] = 1;
         else if (op != OP_CHECK) defined[ins[1]] = 1;
     }
-    if (!checked && !stored) return fail(c, MS_ERR_INVALID, "%s: program stores no result", who);
+    for (unsigned s = 0; s < stored.size(); s++) {
+        if (stored[s]) continue;
+        if (nout == 1) return fail(c, MS_ERR_INVALID, "%s: program stores no result", who);
+        return fail(c, MS_ERR_INVALID, "%s: program never stores slot %u of %u", who, s, nout);
+    }
     return MS_OK;
 }
 

@@ -13,45 +13,9 @@
 //   3. every CTA re-reads its tile, scans the thread aggregates again, applies tile prefix ∘ thread prefix
 //      to `init` and walks its 8 rows writing x_i (exclusive) or x_(i+1) (inclusive).
 // Traffic: a and b are read twice, out written once; the arithmetic is Fq3 (or Fp) multiplications.
-#include "ctx.cuh"
+#include "scan.cuh"
 
 namespace ms {
-
-using gl::Fq3;
-
-template <int L>
-struct El;
-template <>
-struct El<1> {
-    u64 v;
-    __device__ __forceinline__ static El one() { return El{gl::ONE}; }
-    __device__ __forceinline__ static El zero() { return El{0}; }
-    __device__ __forceinline__ static El load(const u64 *p, int f, size_t i) { (void)f; return El{p[i]}; }
-    __device__ __forceinline__ void store(u64 *p, size_t i) const { p[i] = v; }
-    __device__ __forceinline__ El mul(El o) const { return El{gl::mul(v, o.v)}; }
-    __device__ __forceinline__ El add(El o) const { return El{gl::add(v, o.v)}; }
-};
-template <>
-struct El<3> {
-    Fq3 v;
-    __device__ __forceinline__ static El one() { return El{Fq3{gl::ONE, 0, 0}}; }
-    __device__ __forceinline__ static El zero() { return El{Fq3{0, 0, 0}}; }
-    __device__ __forceinline__ static El load(const u64 *p, int f, size_t i) {
-        return f == 1 ? El{Fq3{p[i], 0, 0}} : El{Fq3{p[3 * i], p[3 * i + 1], p[3 * i + 2]}};
-    }
-    __device__ __forceinline__ void store(u64 *p, size_t i) const { p[3 * i] = v.c0; p[3 * i + 1] = v.c1; p[3 * i + 2] = v.c2; }
-    __device__ __forceinline__ El mul(El o) const { return El{gl::mul(v, o.v)}; }
-    __device__ __forceinline__ El add(El o) const { return El{gl::add(v, o.v)}; }
-};
-
-template <int L>
-struct Map {      // x -> x*a + b
-    El<L> a, b;
-    __device__ __forceinline__ static Map identity() { return Map{El<L>::one(), El<L>::zero()}; }
-    // this first, then o
-    __device__ __forceinline__ Map then(const Map &o) const { return Map{a.mul(o.a), b.mul(o.a).add(o.b)}; }
-    __device__ __forceinline__ El<L> apply(El<L> x) const { return x.mul(a).add(b); }
-};
 
 struct ScanArgs {
     const u64 *a;      // n elements of field fa, or nullptr
@@ -64,35 +28,12 @@ struct ScanArgs {
     u64 *out;
 };
 
-constexpr int kScanThreads = 256, kScanPerThread = 8, kScanTile = kScanThreads * kScanPerThread;
-
 template <int L>
 __device__ __forceinline__ Map<L> row_map(const ScanArgs &s, const El<L> &ac, size_t i) {
     Map<L> m;
     m.a = s.a ? El<L>::load(s.a, s.fa, i) : ac;
     m.b = s.b ? El<L>::load(s.b, s.fb, i) : El<L>::zero();
     return m;
-}
-
-// inclusive Kogge-Stone scan of one Map per thread; returns this thread's inclusive value, total in sm[T-1]
-template <int L, int T>
-__device__ __forceinline__ Map<L> block_scan(Map<L> mine, Map<L> *sm) {
-    const int tid = threadIdx.x;
-    sm[tid] = mine;
-    __syncthreads();
-#pragma unroll 1
-    for (int d = 1; d < T; d <<= 1) {
-        Map<L> prev;
-        const bool on = tid >= d;
-        if (on) prev = sm[tid - d];
-        __syncthreads();
-        if (on) {
-            mine = prev.then(mine);
-            sm[tid] = mine;
-        }
-        __syncthreads();
-    }
-    return mine;
 }
 
 template <int L>
@@ -106,24 +47,6 @@ __global__ void __launch_bounds__(kScanThreads) scan_tile_aggregate_kernel(ScanA
         if (first + k < s.n) m = m.then(row_map<L>(s, ac, first + k));
     block_scan<L, kScanThreads>(m, sm);
     if (threadIdx.x == 0) agg[blockIdx.x] = sm[kScanThreads - 1];
-}
-
-// exclusive prefixes of the tile aggregates, in place (one CTA; each thread owns a contiguous chunk)
-template <int L>
-__global__ void __launch_bounds__(1024) scan_tile_prefix_kernel(Map<L> *agg, size_t ntiles) {
-    extern __shared__ unsigned char scan_sm_raw[];
-    Map<L> *sm = reinterpret_cast<Map<L> *>(scan_sm_raw);
-    const size_t chunk = (ntiles + 1023) / 1024;
-    const size_t lo = (size_t)threadIdx.x * chunk, hi = lo + chunk < ntiles ? lo + chunk : ntiles;
-    Map<L> m = Map<L>::identity();
-    for (size_t t = lo; t < hi; t++) m = m.then(agg[t]);
-    block_scan<L, 1024>(m, sm);
-    Map<L> run = threadIdx.x ? sm[threadIdx.x - 1] : Map<L>::identity();
-    for (size_t t = lo; t < hi; t++) {
-        const Map<L> cur = agg[t];
-        agg[t] = run;
-        run = run.then(cur);
-    }
 }
 
 template <int L>

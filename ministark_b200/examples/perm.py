@@ -9,13 +9,17 @@ Fq3 composition trace, Fq3 DEEP and Fq3 FRI.
 
     base columns       0: a      1: b = a shuffled      2: c = a^4
     extension columns  3: op (running product over a)   4: sp (running product over b)
+
+PermAirConfig leaves the extension columns to the trace's host callback (gen_trace); PermDeclaredAirConfig has the same
+constraints and declares the two running products instead (AirConfig.extension_columns), so that the prover builds them
+on the device from a base-only trace (gen_trace(..., extension=False)).
 """
 import random
 
 import numpy as np
 
 from .. import expr as E
-from ..air import AirConfig, domain_generator
+from ..air import AirConfig, RunningColumn, domain_generator
 from ..prover import Stark, Trace
 
 P = E.P
@@ -47,7 +51,18 @@ class PermAirConfig(AirConfig):
         ]
 
 
-def gen_trace(n, seed=1):
+class PermDeclaredAirConfig(PermAirConfig):
+    """PermAirConfig with its extension columns declared: op_0 = sp_0 = 1, op_(i+1) = op_i * (alpha - a_i),
+    sp_(i+1) = sp_i * (alpha - b_i) — what gen_trace's callback computes, row by row on the host"""
+
+    @staticmethod
+    def extension_columns(trace_len):
+        alpha, a, b = E.Challenge(0), E.Trace(0, 0), E.Trace(1, 0)
+        return [RunningColumn(init=1, mul=alpha - a), RunningColumn(init=1, mul=alpha - b)]
+
+
+def gen_trace(n, seed=1, extension=True):
+    """the perm trace of n rows; extension=False: base columns only (for PermDeclaredAirConfig)"""
     rng = random.Random(seed)
     a = [rng.randrange(P) for _ in range(n)]
     b = list(a)
@@ -55,7 +70,7 @@ def gen_trace(n, seed=1):
     c = [pow(v, 4, P) for v in a]
     base = np.array([[v * _R % P for v in col] for col in (a, b, c)], dtype=np.uint64)
 
-    def extension(challenges):
+    def build_extension(challenges):
         alpha = tuple(challenges[0])
         cols = []
         for src in (a, b):
@@ -66,7 +81,7 @@ def gen_trace(n, seed=1):
             cols.append([w * _R % P for w in out])
         return np.array(cols, dtype=np.uint64)
 
-    return Trace(base, extension)
+    return Trace(base, build_extension if extension else None)
 
 
 class PermClaim(Stark):
@@ -74,3 +89,7 @@ class PermClaim(Stark):
 
     def get_public_inputs(self):
         return []
+
+
+class PermDeclaredClaim(PermClaim):
+    AirConfig = PermDeclaredAirConfig

@@ -324,32 +324,10 @@ def _batch_inverses(root, num_base_cols):
     return rebuilt[id(root)]
 
 
-def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, log_ce=None, fold_pow0=True, symbolic=False,
-                    num_cols=None, max_live_leaves=None, batch_inverses=False):
-    """Flatten `expr` into the evaluator's linear program.
-
-    batch_inverses: see _batch_inverses — for programs whose denominators cannot vanish on the evaluation domain (the
-    AIR composition and DEEP programs built by air.py).
-
-    max_live_leaves: keep at most this many leaf values (trace cells, constants, x) in registers; beyond it the least
-    recently used one is dropped and loaded again at its next use.  A sum that names every column twice (the grouped
-    DEEP expression, deep.py) then runs in a dozen registers instead of one per column.
-
-    num_cols: total number of trace columns (base + extension); periodic tables take the column slots after them
-    (required when the expression has Periodic leaves).
-
-    symbolic=True keeps Challenge / Hint / CompositionCoeff leaves as run-time constants (Program.bind fills them in)
-    instead of folding their values into the program: compile once per AIR, bind per proof.
-
-    challenges / hints: extension elements as 3-tuples (or ints) of canonical integers, substituted
-    as constants exactly like eval_cpu.rs:116-118.  Trace(col, off) with col < num_base_cols reads a
-    base-field column, otherwise extension column col - num_base_cols; the row shift is
-    lde_step * off (eval_cpu.rs:119-123).  The result is always stored as an Fq element.
-    """
-    trace_len = (1 << log_ce) // lde_step if log_ce is not None and lde_step >= 1 else 0
-
-    # a / b  ->  a * inv(b) with inv(b) hash-consed, so a denominator shared by many constraints
-    # (the zerofier X^n - 1) is inverted once per point instead of once per Div node
+def _rewrite(roots, trace_len):
+    """the evaluator's form of the DAG under `roots` (one memo for all of them, so shared nodes stay shared): a / b becomes
+    a * inv(b) with inv(b) hash-consed, so a denominator shared by many constraints (the zerofier X^n - 1) is inverted
+    once per point instead of once per Div node; with trace_len, degree adjustments x^(a n + b) become (x^n)^a * x^b"""
     rewritten = {}
 
     def rewrite(e):
@@ -381,13 +359,51 @@ def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, lo
             stack.pop()
         return rewritten[id(e)]
 
-    expr = rewrite(expr)
+    return [rewrite(e) for e in roots]
+
+
+def compile_program(expr, num_base_cols, challenges=(), hints=(), lde_step=1, log_ce=None, fold_pow0=True, symbolic=False,
+                    num_cols=None, max_live_leaves=None, batch_inverses=False):
+    """Flatten `expr` into the evaluator's linear program.
+
+    batch_inverses: see _batch_inverses — for programs whose denominators cannot vanish on the evaluation domain (the
+    AIR composition and DEEP programs built by air.py).
+
+    max_live_leaves: keep at most this many leaf values (trace cells, constants, x) in registers; beyond it the least
+    recently used one is dropped and loaded again at its next use.  A sum that names every column twice (the grouped
+    DEEP expression, deep.py) then runs in a dozen registers instead of one per column.
+
+    num_cols: total number of trace columns (base + extension); periodic tables take the column slots after them
+    (required when the expression has Periodic leaves).
+
+    symbolic=True keeps Challenge / Hint / CompositionCoeff leaves as run-time constants (Program.bind fills them in)
+    instead of folding their values into the program: compile once per AIR, bind per proof.
+
+    challenges / hints: extension elements as 3-tuples (or ints) of canonical integers, substituted
+    as constants exactly like eval_cpu.rs:116-118.  Trace(col, off) with col < num_base_cols reads a
+    base-field column, otherwise extension column col - num_base_cols; the row shift is
+    lde_step * off (eval_cpu.rs:119-123).  The result is always stored as an Fq element.
+    """
+    trace_len = (1 << log_ce) // lde_step if log_ce is not None and lde_step >= 1 else 0
+    expr = _rewrite([expr], trace_len)[0]
     if batch_inverses:
         expr = _batch_inverses(expr, num_base_cols)
     code, consts, nregs, typ, bindings, periodic = _lower(
         [expr], lambda k, r, t: [OP_STORE | (t << 8), 0, r, 0], num_base_cols, challenges, hints, lde_step, log_ce, symbolic,
         num_cols, max_live_leaves)
     return Program(code, consts, nregs, typ[id(expr)] == FQ, bindings, periodic)
+
+
+def compile_extension_program(muls, adds, num_base_cols, log_n, num_cols):
+    """Flatten the row maps of K declared extension columns (air.RunningColumn) into ONE evaluator program for
+    csrc/extension.cu: mul_k is stored to slot 2k and add_k to slot 2k + 1, subexpressions shared between them are computed
+    once per row.  Trace(col, off) reads column[(i + off) mod 2^log_n] of the natural-order trace; X is g_n^i; periodic
+    tables come from periodic_tables(ctx, program, log_n, 1, offset_canonical=1).  Challenges and hints stay symbolic
+    (Program.bind).  Division is a * inv(b), and the inverse of zero is zero, on the device and in host folding alike."""
+    roots = _rewrite([Expr._lift(r) for pair in zip(muls, adds) for r in pair], 0)
+    code, consts, nregs, _, bindings, periodic = _lower(
+        roots, lambda k, r, t: [OP_STORE | (t << 8), k, r, 0], num_base_cols, (), (), 1, log_n, True, num_cols, None)
+    return Program(code, consts, nregs, True, bindings, periodic)
 
 
 def compile_check_program(constraints, num_base_cols, log_n, num_cols, symbolic=True, challenges=(), hints=()):

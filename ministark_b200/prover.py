@@ -32,7 +32,7 @@ from . import FP, FQ3, GENERATOR as GEN_MONT, ONE, Context
 from . import deep
 from . import expr as E
 from . import verifier
-from .air import Air
+from .air import Air, _leaves
 from .channel import ProverChannel, PublicCoin, serialize_element
 from .cosets import block_program, coset_offsets, heap_location, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
@@ -77,6 +77,36 @@ class Trace:
 
     def build_extension_columns(self, challenges):
         return None if self._ext is None else self._ext(challenges)
+
+
+def declared_extension_columns(ctx, air, challenges, hints, base, device):
+    """the extension columns `air` declares (AirConfig.extension_columns), built on the device from the natural-order base
+    columns `base` ((NUM_BASE_COLUMNS, n) device tensor) by ms_extension_columns: the cached program bound with this
+    proof's challenges and hints, each init evaluated on the host.  Returns a (K, n * fq) device tensor."""
+    cfg = air.config
+    fq = FP if cfg.FQ_IS_FP else FQ3
+    decl, prog = air.extension_declaration, air.extension_program()
+    for k, c in enumerate(decl):
+        for e in (c.init, c.mul, c.add):
+            for (i,) in sorted(_leaves(e, "hint")):
+                if i >= len(hints):
+                    raise ProvingError(f"extension column {cfg.NUM_BASE_COLUMNS + k} reads Hint({i}), but gen_hints "
+                                       f"returned {len(hints)} hints")
+    prog = prog.bind(challenges=challenges, hints=hints)
+    init = np.array([[_mont(w) for w in E.evaluate_at(c.init, 0, challenges=challenges, hints=hints)[:fq]] for c in decl],
+                    dtype=np.uint64)
+    n = air.trace_len
+    out = torch.empty((len(decl), n * fq), dtype=torch.int64, device=device)
+    tables = E.periodic_tables(ctx, prog, air.log_n, 1, offset_canonical=1)
+    try:
+        ctx.extension_columns(prog, out, air.log_n, [base[c] for c in range(cfg.NUM_BASE_COLUMNS)] + [p for p, _ in tables],
+                              [False] * cfg.NUM_BASE_COLUMNS + [q for _, q in tables], fq, init, [c.inclusive for c in decl])
+    finally:
+        if tables:
+            ctx.sync()
+        for p, _ in tables:
+            ctx.free(p)
+    return out
 
 
 class _Tree:
@@ -340,6 +370,7 @@ class GpuProver:
             self._airs[key] = Air(cfg, n, None, options)
             self._airs[key].composition_program()
             self._airs[key].deep_program()
+            self._airs[key].extension_program()
             self._airs[key].num_challenges(), self._airs[key].num_composition_constraint_coeffs(), self._airs[key].trace_arguments()
         air = copy.copy(self._airs[key])
         air.public_inputs = stark.get_public_inputs()
@@ -407,7 +438,7 @@ class GpuProver:
         hints = air.gen_hints(challenges)
 
         # ---- extension trace commitment (prover.rs:56-72)
-        ext = self._extension_columns(r, challenges, base)
+        ext = self._extension_columns(r, challenges, hints, base)
         check = self._keep_for_check(r, base, ext)
         del base
         ext_polys = ext_lde = ext_tree = None
@@ -543,7 +574,7 @@ class GpuProver:
         hints = air.gen_hints(challenges)
 
         # ---- extension trace commitment
-        ext = self._extension_columns(r, challenges, base)
+        ext = self._extension_columns(r, challenges, hints, base)
         check = self._keep_for_check(r, base, ext)
         del base
         ext_polys = ext_blk = ext_nodes = None
@@ -636,12 +667,15 @@ class GpuProver:
             r.stark.validate_constraints(r.air, challenges, hints, check[0], check[1], r.ctx)
             r.lap("validate_constraints")
 
-    def _extension_columns(self, r, challenges, base):
+    def _extension_columns(self, r, challenges, hints, base):
+        """the trace's own builder first (device or host); without one, the columns the AIR declares, built on the device"""
         if hasattr(r.trace, "build_extension_columns_device"):
             # running products / evaluations as device scans over the resident base trace (SURVEY.md §8f rank 3)
             ext = r.trace.build_extension_columns_device(challenges, r.ctx, base)
         else:
             ext = r.trace.build_extension_columns(challenges)
+            if ext is None and r.air.extension_declaration:
+                ext = declared_extension_columns(r.ctx, r.air, challenges, hints, base, self.device)
         release = getattr(r.trace, "release_base_columns", None)
         if release is not None:     # the natural-order base matrix is not read from the trace again in this proof
             release()

@@ -36,7 +36,7 @@ from .air import domain_generator
 from .channel import ProverChannel
 from .cosets import block_program, brev as _brev, coset_offsets, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
-from .prover import GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont
+from .prover import GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont, declared_extension_columns
 
 P = E.P
 _R = 2**64
@@ -318,6 +318,7 @@ class ShardedProver(GpuProver):
             air0 = Air(cfg, n, None, options)
             air0.composition_program()
             air0.deep_program()
+            air0.extension_program()
             block_program(air0)              # the composition evaluated block by block
             air0.num_challenges(), air0.num_composition_constraint_coeffs(), air0.trace_arguments()
             self._airs[key] = air0
@@ -354,11 +355,14 @@ class ShardedProver(GpuProver):
         challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
         hints = air.gen_hints(challenges)
 
-        # ---- extension trace commitment (prover.rs:56-72): built from the (replicated) base trace on every rank
+        # ---- extension trace commitment (prover.rs:56-72): built from the (replicated) base trace on every rank, by the
+        # trace's own builder or, without one, from the AIR's declaration
         if hasattr(trace, "build_extension_columns_device"):
             ext = trace.build_extension_columns_device(challenges, ctx, base)
         else:
             ext = trace.build_extension_columns(challenges)
+            if ext is None and air.extension_declaration:
+                ext = declared_extension_columns(ctx, air, challenges, hints, base, self.device)
         del base
         num_ext = 0 if ext is None else int(ext.shape[0])
         if num_ext != next_:
