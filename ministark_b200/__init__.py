@@ -339,6 +339,33 @@ class Context:
                                                program.consts.shape[0], ptrs, isq, k, fq_field, log_n, len(inclusive),
                                                ini.ctypes.data, inc, _ptr(out)))
 
+    def lookup_workspace_bytes(self, log_n, width, ntuples):
+        """bytes of the workspace lookup_multiplicities needs (ms_lookup_workspace_bytes; arithmetic only)"""
+        out = C.c_size_t()
+        rc = self.lib.ms_lookup_workspace_bytes(log_n, width, ntuples, C.byref(out))
+        if rc != 0:
+            raise MsError(f"[{rc}] ms_lookup_workspace_bytes: log_n={log_n}, width={width}, ntuples={ntuples} out of range")
+        return int(out.value)
+
+    def lookup_multiplicities(self, program, out, log_n, cols, width, ntuples, workspace):
+        """the multiplicity column of one LogUp lookup (include/ministark_lookup.h) into `out` (2^log_n Montgomery words on
+        the device): `program` from expr.compile_lookup_program, `cols`: natural-order base columns (device), then the
+        program's periodic tables; workspace: a device buffer of lookup_workspace_bytes(log_n, width, ntuples) bytes.
+        Returns (missing, bad): per value tuple (number of rows whose tuple is not in the table, lowest such row), and
+        (number of (row, tuple) pairs whose selector is neither 0 nor 1, lowest such row); a lowest row is None where
+        there is none."""
+        k = len(cols)
+        ptrs = (C.c_void_p * max(k, 1))(*[_ptr(c) for c in cols])
+        isq = (C.c_int * max(k, 1))()
+        status = np.zeros(2 * ntuples + 2, dtype=np.uint64)
+        nbytes = workspace.numel() * workspace.element_size() if hasattr(workspace, "numel") else workspace.nbytes
+        self._ck(self.lib.ms_lookup_multiplicities(self.h, program.code.ctypes.data, len(program), program.consts.ctypes.data,
+                                                   program.consts.shape[0], ptrs, isq, k, log_n, width, ntuples,
+                                                   _ptr(workspace), nbytes, _ptr(out), status.ctypes.data))
+        pairs = [(int(status[2 * q]), None if int(status[2 * q + 1]) == 2**64 - 1 else int(status[2 * q + 1]))
+                 for q in range(ntuples + 1)]
+        return pairs[:ntuples], pairs[ntuples]
+
     def poly_eval(self, coeffs, field, n, ncols, points, col_stride=None):
         """horner_evaluate of every column at every point (get_ood_evals, src/composer.rs:43-86).
         points: (k, 3) Montgomery words; returns (ncols, k, 3) numpy uint64."""

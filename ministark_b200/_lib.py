@@ -13,6 +13,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_b200.h"
 STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_stream.h")
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
 EXTENSION_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_extension.h")
+LOOKUP_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_lookup.h")
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
@@ -86,6 +87,12 @@ _EXTENSION_SIGS = {
     "ms_extension_columns": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ci, ui, ui, vp, vp, vp]),
 }
 
+# include/ministark_lookup.h: multiplicity columns of the LogUp lookups an AIR declares (air.Lookup), filled on the device
+_LOOKUP_SIGS = {
+    "ms_lookup_workspace_bytes": (ci, [ui, ui, ui, C.POINTER(sz)]),
+    "ms_lookup_multiplicities": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ui, ui, ui, vp, sz, vp, vp]),
+}
+
 # include/ministark_bf.h: the execution trace of examples/brainfuck (VM on the host, tables on the device)
 _BF_SIGS = {
     "ms_bf_run": (ci, [vp, sz, vp, sz, u64, vp, vp, vp]),
@@ -134,6 +141,7 @@ def load():
         bind(lib, _STREAM_SIGS)
         bind(lib, _CHECK_SIGS)
         bind(lib, _EXTENSION_SIGS)
+        bind(lib, _LOOKUP_SIGS)
         bind(lib, _BF_SIGS)
         bind(lib, _DEVICE_SIGS)
         bind(lib, _HOST_NODES_SIGS)

@@ -171,6 +171,43 @@ def _as_expr(v):
     return E.Constant(tuple(v)) if isinstance(v, (tuple, list)) else E.Constant(v)
 
 
+MAX_LOOKUP_WIDTH = 4                             # csrc/lookup.cu: at most this many words per tuple
+MAX_LOOKUP_TUPLES = 4                            # and this many value tuples per lookup
+
+
+@dataclass(frozen=True)
+class Lookup:
+    """One LogUp lookup (AirConfig.lookups): at every row i where selectors[q](i) == 1 (every row without selectors), the
+    tuple values[q] at row i is a row of the table, the tuple `table` at row j for j = 0..n-1.  Every row of `table` is a
+    table entry; pad a short table by repeating a real entry.
+
+    table: W Exprs (or Fp values), values: Q tuples of W Exprs, selectors: None or Q Exprs, 1 <= W, Q <= 4.  They read
+    Constant (Fp), X, Periodic and Trace(c, offset) of a base column c at any offset (the row index wraps mod n); never a
+    challenge, a hint, an extension column or a multiplicity column, since the multiplicities are filled before the base
+    trace is committed.
+
+    multiplicity: a base column the prover writes: row j holds the number of (row, value tuple) pairs that look up the
+    table tuple at row j; a tuple that occurs more than once in the table counts at its lowest row only, the others get 0.
+    running_sum: an extension column the package declares and constrains.  AirConfig.extension_columns returns None at
+    its position.
+
+    Challenges: with c0 the number of challenges the AIR's own constraints draw, lookup l (in declaration order) takes the
+    next index as alpha_l, and one more as beta_l only when W > 1.  Tuples are compressed as t_0 + beta t_1 + beta^2 t_2 +
+    ..., and d_0 = alpha - (table tuple), d_q = alpha - (value tuple q).  The running sum is s_0 = 0,
+    s_(i+1) = s_i + m_i / d_0 - sum_q sigma_q / d_q (sigma_q: the selector, 1 without one), and three constraints are
+    appended after the AIR's own, per lookup: s_0 = 0, the step with its denominators cleared on every row but the last,
+    and the whole sum being zero at the last row.
+
+    Soundness: the multiplicity fill is untrusted prover work; the generated constraints are what make a proof a proof of
+    the lookup.  The package does not constrain a selector to {0, 1}: if it is a witness column, the AIR must.  With
+    FQ_IS_FP = True alpha is drawn from the 64-bit base field, and the argument's soundness error is about (Q + 1) n / p."""
+    table: tuple
+    values: tuple
+    multiplicity: int
+    running_sum: int
+    selectors: tuple = None
+
+
 class AirConfig:
     """Subclass and override, as with the reference's trait (src/air.rs:26-48).  Field values handed to and
     returned by the hooks are canonical integers (Fp) or 3-tuples of canonical integers (Fq3)."""
@@ -194,8 +231,16 @@ class AirConfig:
     def extension_columns(trace_len):
         """None (the trace builds its own extension columns), or one RunningColumn per extension column, in column
         order: the prover then builds them on the device from the base trace whenever the trace brings no builder of its
-        own.  A declaration adds no constraint: the AIR's constraints must still enforce every declared column."""
+        own.  A declaration adds no constraint: the AIR's constraints must still enforce every declared column.  With
+        lookups: None at every lookup's running-sum position (the package declares those columns), or None as a whole
+        when every extension column is a lookup's running sum."""
         return None
+
+    @staticmethod
+    def lookups(trace_len):
+        """the AIR's LogUp lookups (Lookup), in declaration order.  The package generates their constraints and
+        running-sum columns, and the prover fills their multiplicity columns on the device."""
+        return []
 
 
 class Air:
@@ -206,6 +251,9 @@ class Air:
         self.config, self.trace_len, self.public_inputs, self.options = config, trace_len, public_inputs, options
         self.log_n = trace_len.bit_length() - 1
         self.constraints = list(config.constraints(trace_len))
+        hook = getattr(config, "lookups", None)
+        self.lookups = self._lookups(list(hook(trace_len)) if hook is not None else [])
+        self.constraints += self._lookup_constraints()
         # AirConfig::composition_constraint (src/air.rs:50-82)
         ce_blowup = max(blowup_factor(c, trace_len) for c in self.constraints)
         composition_degree = trace_len * ce_blowup - 1
@@ -223,7 +271,139 @@ class Air:
         self.ce_blowup_factor = blowup_factor(total, trace_len)
         assert self.ce_blowup_factor <= options.lde_blowup_factor
         hook = getattr(config, "extension_columns", None)
-        self.extension_declaration = self._declaration(hook(trace_len) if hook is not None else None)
+        self.extension_declaration = self._declaration(self._merge_lookup_sums(hook(trace_len) if hook is not None else None))
+
+    def _lookups(self, decl):
+        """AirConfig.lookups checked against the AIR: Lookups with Expr fields, or ValueError.  Also assigns each lookup its
+        challenges (self.lookup_challenges: (alpha index, beta index or None))"""
+        cfg = self.config
+        nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
+        idx = [a[0] for c in self.constraints for a in _leaves(c, "chal")]
+        chal = max(idx) + 1 if idx else 0
+        out, self.lookup_challenges = [], []
+        mults, sums = {}, {}
+        for l, lk in enumerate(decl):
+            if not isinstance(lk, Lookup):
+                raise ValueError(f"lookup {l}: expected a Lookup, got {type(lk).__name__}")
+            m, s = lk.multiplicity, lk.running_sum
+            if not 0 <= m < nbase:
+                raise ValueError(f"lookup {l}: multiplicity column {m} is not a base column (0..{nbase - 1})")
+            if m in mults:
+                raise ValueError(f"lookup {l}: multiplicity column {m} is also lookup {mults[m]}'s")
+            if not nbase <= s < nbase + next_:
+                raise ValueError(f"lookup {l}: running-sum column {s} is not an extension column ({nbase}..{nbase + next_ - 1})")
+            if s in sums:
+                raise ValueError(f"lookup {l}: running-sum column {s} is also lookup {sums[s]}'s")
+            mults[m], sums[s] = l, l
+            table, values = tuple(lk.table), tuple(tuple(v) for v in lk.values)
+            W, Q = len(table), len(values)
+            if not 1 <= W <= MAX_LOOKUP_WIDTH:
+                raise ValueError(f"lookup {l}: table tuples of width {W}; 1 to {MAX_LOOKUP_WIDTH} are supported")
+            if not 1 <= Q <= MAX_LOOKUP_TUPLES:
+                raise ValueError(f"lookup {l}: {Q} value tuples; 1 to {MAX_LOOKUP_TUPLES} are supported")
+            for q, v in enumerate(values):
+                if len(v) != W:
+                    raise ValueError(f"lookup {l}: value tuple {q} has width {len(v)}, the table {W}")
+            sel = None if lk.selectors is None else tuple(lk.selectors)
+            if sel is not None and len(sel) != Q:
+                raise ValueError(f"lookup {l}: {len(sel)} selectors for {Q} value tuples")
+            out.append(Lookup(tuple(_as_expr(t) for t in table), tuple(tuple(_as_expr(w) for w in v) for v in values), m, s,
+                              None if sel is None else tuple(_as_expr(e) for e in sel)))
+            self.lookup_challenges.append((chal, chal + 1 if W > 1 else None))
+            chal += 2 if W > 1 else 1
+        for l, lk in enumerate(out):
+            named = [(f"table[{k}]", e) for k, e in enumerate(lk.table)]
+            named += [(f"values[{q}][{k}]", e) for q, v in enumerate(lk.values) for k, e in enumerate(v)]
+            named += [(f"selectors[{q}]", e) for q, e in enumerate(lk.selectors or ())]
+            for name, e in named:
+                for kind, what in (("chal", "a challenge"), ("hint", "a hint"), ("ccoef", "a composition coefficient")):
+                    if _leaves(e, kind):
+                        raise ValueError(f"lookup {l}: {name} reads {what}")
+                if any(ext for _, ext in _leaves(e, "const")):
+                    raise ValueError(f"lookup {l}: {name} reads an extension-field constant")
+                for col, off in sorted(_leaves(e, "trace")):
+                    if col in mults:
+                        raise ValueError(f"lookup {l}: {name} reads Trace({col}, {off}), the multiplicity column of lookup "
+                                         f"{mults[col]}")
+                    if not 0 <= col < nbase:
+                        raise ValueError(f"lookup {l}: {name} reads Trace({col}, {off}), which is not a base column "
+                                         f"(0..{nbase - 1})")
+        return out
+
+    def _compressed(self, l, tup):
+        """t_0 + beta t_1 + beta^2 t_2 + ... with lookup l's beta"""
+        acc = tup[0]
+        b = self.lookup_challenges[l][1]
+        bpow = None
+        for t in tup[1:]:
+            bpow = E.Challenge(b) if bpow is None else bpow * E.Challenge(b)
+            acc = acc + bpow * t
+        return acc
+
+    def _lookup_denominators(self, l):
+        lk = self.lookups[l]
+        alpha = E.Challenge(self.lookup_challenges[l][0])
+        return [alpha - self._compressed(l, lk.table)] + [alpha - self._compressed(l, v) for v in lk.values]
+
+    def _lookup_constraints(self):
+        """the three constraints of every lookup (Lookup), appended after the AIR's own.  With Q = 1, W = 1 and no selectors
+        they are, node for node, the LogUp constraints examples/lookup.py's LookupAirConfig writes by hand."""
+        n = self.trace_len
+        g = domain_generator(self.log_n)
+        x, one = E.X(), E.Constant(1)
+        first, last = E.Constant(1), E.Constant(pow(g, n - 1, P))
+        but_last = (x - last) / (x ** n - one)
+        out = []
+        for l, lk in enumerate(self.lookups):
+            d = self._lookup_denominators(l)
+            Q = len(lk.values)
+            m, s, s1 = E.Trace(lk.multiplicity, 0), E.Trace(lk.running_sum, 0), E.Trace(lk.running_sum, 1)
+            num = m
+            for dq in d[1:]:
+                num = num * dq
+            for q in range(1, Q + 1):
+                term = None
+                for r in range(Q + 1):
+                    if r != q:
+                        term = d[r] if term is None else term * d[r]
+                if lk.selectors is not None:
+                    term = lk.selectors[q - 1] * term
+                num = num - term
+            step, total = s1 - s, s
+            for dq in d:
+                step, total = step * dq, total * dq
+            out += [s / (x - first), (step - num) * but_last, (total + num) / (x - last)]
+        return out
+
+    def _merge_lookup_sums(self, decl):
+        """the user's extension_columns with every lookup's running sum put in its place (RunningColumn(init=0,
+        add=m / d_0 - sum_q sigma_q / d_q)), or ValueError"""
+        if not self.lookups:
+            return decl
+        cfg = self.config
+        nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
+        pos = {lk.running_sum - nbase: l for l, lk in enumerate(self.lookups)}
+        if decl is None:
+            if len(pos) != next_:
+                raise ValueError(f"extension_columns returned None, but only {len(pos)} of the {next_} extension columns "
+                                 f"are lookup running sums")
+            decl = [None] * next_
+        decl = list(decl)
+        if len(decl) != next_:
+            raise ValueError(f"extension_columns declares {len(decl)} columns but NUM_EXTENSION_COLUMNS is {next_}")
+        for k, col in enumerate(decl):
+            if k in pos and col is not None:
+                raise ValueError(f"extension column {nbase + k}: lookup {pos[k]}'s running sum is declared by the package; "
+                                 f"extension_columns must return None there")
+            if k not in pos and not isinstance(col, RunningColumn):
+                raise ValueError(f"extension column {nbase + k}: expected a RunningColumn, got {type(col).__name__}")
+        for k, l in pos.items():
+            lk, d = self.lookups[l], self._lookup_denominators(l)
+            add = E.Trace(lk.multiplicity, 0) / d[0]
+            for q, dq in enumerate(d[1:]):
+                add = add - (E.Constant(1) if lk.selectors is None else lk.selectors[q]) / dq
+            decl[k] = RunningColumn(init=0, add=add)
+        return decl
 
     def _declaration(self, decl):
         """AirConfig.extension_columns checked against the AIR: RunningColumns with Expr fields, or ValueError"""
@@ -304,6 +484,14 @@ class Air:
                                                                   self.config.NUM_BASE_COLUMNS, self.log_n,
                                                                   self.config.NUM_BASE_COLUMNS)
         return getattr(self, "_extension_program", None)
+
+    def lookup_programs(self):
+        """one evaluator program per lookup, for its multiplicity fill (csrc/lookup.cu, expr.compile_lookup_program)"""
+        if getattr(self, "_lookup_programs", None) is None:
+            nbase = self.config.NUM_BASE_COLUMNS
+            self._lookup_programs = [E.compile_lookup_program(lk.table, lk.values, lk.selectors, nbase, self.log_n)
+                                     for lk in self.lookups]
+        return self._lookup_programs
 
     # the three walks below depend on the constraints only: done once per Air (the provers copy a cached Air per proof,
     # and each walk of the brainfuck AIR costs ~0.5 ms of a 10 ms proof)

@@ -406,6 +406,30 @@ def compile_extension_program(muls, adds, num_base_cols, log_n, num_cols):
     return Program(code, consts, nregs, True, bindings, periodic)
 
 
+def lookup_slots(width, ntuples):
+    """the output slots of a lookup program: the table words 0..W-1, then per value tuple q its selector at
+    W + q (W + 1) and its words right after it"""
+    return width + ntuples * (width + 1)
+
+
+def compile_lookup_program(table, values, selectors, num_base_cols, log_n):
+    """Flatten one lookup (air.Lookup) into ONE evaluator program for csrc/lookup.cu: table word k is stored to slot k,
+    value tuple q's selector (Constant 1 without selectors) to slot W + q (W + 1) and its word k to the slot k + 1 after
+    that.  Every expression is over the base field: Trace(col, off) reads column[(i + off) mod 2^log_n] of the
+    natural-order trace, X is g_n^i, periodic tables come from periodic_tables(ctx, program, log_n, 1,
+    offset_canonical=1)."""
+    W = len(table)
+    roots = [Expr._lift(t) for t in table]
+    for q, v in enumerate(values):
+        roots.append(Constant(1) if selectors is None else Expr._lift(selectors[q]))
+        roots += [Expr._lift(w) for w in v]
+    assert len(roots) == lookup_slots(W, len(values))
+    roots = _rewrite(roots, 0)
+    code, consts, nregs, _, bindings, periodic = _lower(
+        roots, lambda k, r, t: [OP_STORE | (t << 8), k, r, 0], num_base_cols, (), (), 1, log_n, True, num_base_cols, None)
+    return Program(code, consts, nregs, False, bindings, periodic)
+
+
 def compile_check_program(constraints, num_base_cols, log_n, num_cols, symbolic=True, challenges=(), hints=()):
     """Flatten every constraint into ONE checked program for csrc/check.cu, which runs Constraint::check
     (src/constraints.rs:168-249) at every row of the trace domain of size 2^log_n: values carry a None flag, Div is the

@@ -24,6 +24,7 @@ import ctypes as C
 import hashlib
 import time
 import weakref
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -32,7 +33,7 @@ from . import FP, FQ3, GENERATOR as GEN_MONT, ONE, Context
 from . import deep
 from . import expr as E
 from . import verifier
-from .air import Air, _leaves
+from .air import Air, _leaves, domain_generator
 from .channel import ProverChannel, PublicCoin, serialize_element
 from .cosets import block_program, coset_offsets, heap_location, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
@@ -107,6 +108,98 @@ def declared_extension_columns(ctx, air, challenges, hints, base, device):
         for p, _ in tables:
             ctx.free(p)
     return out
+
+
+@dataclass(frozen=True)
+class LookupMiss:
+    """value tuple `tuple` of lookup `lookup` fails at `count` (row, tuple) pairs, the lowest row being `first_row`:
+    kind "missing": its tuple is not in the table (count: rows of this tuple); kind "selector": its selector is neither 0
+    nor 1 (count: such pairs over all of the lookup's tuples).  values: the tuple at first_row as canonical integers, and
+    the selector for kind "selector"."""
+    lookup: int
+    tuple: int
+    kind: str
+    first_row: int
+    count: int
+    values: tuple
+    selector: int = None
+
+    def message(self):
+        if self.kind == "missing":
+            return (f"lookup {self.lookup}, value tuple {self.tuple}: {self.values} at row {self.first_row} is not in the "
+                    f"table ({self.count} rows of this tuple are not)")
+        return (f"lookup {self.lookup}, value tuple {self.tuple}: the selector is {self.selector} at row {self.first_row}, "
+                f"neither 0 nor 1 ({self.count} (row, tuple) pairs of this lookup have such a selector); the tuple there is "
+                f"{self.values}")
+
+
+class LookupViolation(ProvingError):
+    """a lookup of the AIR does not hold for the trace (raised before anything is committed): `misses` lists one LookupMiss
+    per failing (lookup, value tuple); the message names the first"""
+
+    def __init__(self, misses):
+        self.misses = list(misses)
+        more = f" (and {len(self.misses) - 1} more failing lookup tuples)" if len(self.misses) > 1 else ""
+        super().__init__(self.misses[0].message() + more)
+
+
+def _lookup_misses(ctx, air, base, l, missing, bad):
+    """LookupMiss entries of lookup l from the kernel's status, with the named rows' tuples evaluated on the host from
+    cells gathered off the device"""
+    lk, n, nbase = air.lookups[l], air.trace_len, air.config.NUM_BASE_COLUMNS
+    exprs = [e for v in lk.values for e in v] + list(lk.selectors or ())
+    leaves = sorted(set().union(*(_leaves(e, "trace") for e in exprs)))
+    g = domain_generator(air.log_n)
+
+    def at(row):
+        ids = sorted({(row + off) % n for _, off in leaves})
+        got = ctx.gather_rows(base, FP, n, nbase, ids) if ids else None
+        cells = {(c, off): int(got[ids.index((row + off) % n), c]) * _RINV % P for c, off in leaves}
+        ev = lambda e: E.evaluate_at(e, pow(g, row, P), cells, trace_len=n)[0]
+        return ([tuple(ev(w) for w in v) for v in lk.values],
+                [1] * len(lk.values) if lk.selectors is None else [ev(s) for s in lk.selectors])
+
+    out = []
+    for q, (count, row) in enumerate(missing):
+        if count:
+            vals, _ = at(row)
+            out.append(LookupMiss(l, q, "missing", row, count, vals[q]))
+    if bad[0]:
+        vals, sels = at(bad[1])
+        out += [LookupMiss(l, q, "selector", bad[1], bad[0], vals[q], sels[q]) for q in range(len(sels)) if sels[q] not in (0, 1)]
+    return sorted(out, key=lambda m: (m.tuple, m.kind))
+
+
+def fill_lookup_multiplicities(ctx, air, base):
+    """the multiplicity column of every lookup `air` declares (AirConfig.lookups), written into `base` ((NUM_BASE_COLUMNS,
+    n) natural-order device tensor, the prover's own copy) by ms_lookup_multiplicities, one call per lookup with the
+    cached programs.  Raises LookupViolation if a value tuple is not in its table or a selector is neither 0 nor 1."""
+    nbase, log_n = air.config.NUM_BASE_COLUMNS, air.log_n
+    misses = []
+    for l, (lk, prog) in enumerate(zip(air.lookups, air.lookup_programs())):
+        W, Q = len(lk.table), len(lk.values)
+        work = torch.empty(ctx.lookup_workspace_bytes(log_n, W, Q), dtype=torch.uint8, device=base.device)
+        tables = E.periodic_tables(ctx, prog, log_n, 1, offset_canonical=1)
+        try:
+            missing, bad = ctx.lookup_multiplicities(prog, base[lk.multiplicity], log_n,
+                                                     [base[c] for c in range(nbase)] + [p for p, _ in tables], W, Q, work)
+        finally:
+            for p, _ in tables:
+                ctx.free(p)
+        del work
+        if any(c for c, _ in missing) or bad[0]:
+            misses += _lookup_misses(ctx, air, base, l, missing, bad)
+    if misses:
+        raise LookupViolation(misses)
+
+
+def check_lookup_trace(air, trace):
+    """a trace that builds its own extension columns cannot know the multiplicities the prover fills: refused for an AIR
+    with lookups, before anything is computed"""
+    if air.lookups and (hasattr(trace, "build_extension_columns_device") or getattr(trace, "_ext", None) is not None
+                        or type(trace).build_extension_columns is not Trace.build_extension_columns):
+        raise ProvingError("the AIR declares lookups, whose running sums the package builds from the multiplicities it fills; "
+                           "the trace must not bring its own extension columns")
 
 
 class _Tree:
@@ -273,6 +366,12 @@ class GpuProver:
         a = np.ascontiguousarray(a, dtype=np.uint64)
         return torch.from_numpy(a.view(np.int64)).to(self.device, non_blocking=False)
 
+    def _own_copy(self, a):
+        """a device copy of the (host or device) matrix `a` that shares no memory with it"""
+        if not isinstance(a, torch.Tensor):
+            a = torch.from_numpy(np.ascontiguousarray(a, dtype=np.uint64).view(np.int64))
+        return a.to(self.device, dtype=torch.int64, copy=True).contiguous()
+
     def _empty(self, *shape):
         return torch.empty(shape, dtype=torch.int64, device=self.device)
 
@@ -348,10 +447,14 @@ class GpuProver:
                   "composition_trace_commitment", "deep_composition", "fri", "proof_of_work", "queries"]
         torch.cuda.nvtx.range_push("prove:" + phases[0])
 
-        def lap(name):
+        def lap(name, since=None):
             nonlocal t0
             ctx.sync()
             t = time.perf_counter()
+            if since is not None:           # lookup_multiplicities: timed on its own, outside the phase it runs in
+                timings[name] = t - since
+                t0 += t - since
+                return
             timings[name] = t - t0
             t0 = t
             if name not in phases:          # validate_constraints: timed, outside the fixed phases
@@ -371,9 +474,11 @@ class GpuProver:
             self._airs[key].composition_program()
             self._airs[key].deep_program()
             self._airs[key].extension_program()
+            self._airs[key].lookup_programs()
             self._airs[key].num_challenges(), self._airs[key].num_composition_constraint_coeffs(), self._airs[key].trace_arguments()
         air = copy.copy(self._airs[key])
         air.public_inputs = stark.get_public_inputs()
+        check_lookup_trace(air, trace)
         fq = FP if cfg.FQ_IS_FP else FQ3
         log_n = air.log_n
         beta = options.lde_blowup_factor
@@ -407,7 +512,11 @@ class GpuProver:
         host_base = trace.base_columns()
         if tuple(host_base.shape) != (nbase, n):
             raise ProvingError(f"expected {nbase} base columns of {n} rows")
-        if isinstance(host_base, torch.Tensor) and host_base.is_cuda:
+        if air.lookups:
+            # the multiplicities are filled before the commitment, so the upload cannot overlap the transforms here
+            base = self._lookup_base(r, host_base)
+            base_polys, base_lde, base_tree, base_root = self._commit_columns(base, FP, log_n, log_b, nbase, True)
+        elif isinstance(host_base, torch.Tensor) and host_base.is_cuda:
             base = host_base.to(self.device)
             base_polys, base_lde, base_tree, base_root = self._commit_columns(base, FP, log_n, log_b, nbase, True)
         else:
@@ -562,7 +671,7 @@ class GpuProver:
         host_base = trace.base_columns()
         if tuple(host_base.shape) != (nbase, n):
             raise ProvingError(f"expected {nbase} base columns of {n} rows")
-        base = self._to_device(host_base)
+        base = self._lookup_base(r, host_base) if air.lookups else self._to_device(host_base)
         del host_base                           # held no longer than `base`: see release_base_columns below
         base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
         ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
@@ -653,6 +762,16 @@ class GpuProver:
         return self._finish(r, fri_proof, queries)
 
     # ---- phases both residencies share
+    def _lookup_base(self, r, host_base):
+        """the prover's own device copy of the base columns (the caller's trace, host or device, is never written) with
+        every lookup's multiplicity column filled; timed as timings["lookup_multiplicities"]"""
+        base = self._own_copy(host_base)
+        r.ctx.sync()
+        t = time.perf_counter()
+        fill_lookup_multiplicities(r.ctx, r.air, base)
+        r.lap("lookup_multiplicities", since=t)
+        return base
+
     def _keep_for_check(self, r, base, ext):
         """with validation: the natural-order base columns and the extension columns on the device (a host-built
         extension matrix uploaded once, for the check and the commitment), kept until the check has run"""

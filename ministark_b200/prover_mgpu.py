@@ -36,7 +36,8 @@ from .air import domain_generator
 from .channel import ProverChannel
 from .cosets import block_program, brev as _brev, coset_offsets, merkle_walk
 from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
-from .prover import GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont, declared_extension_columns
+from .prover import (GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont, check_lookup_trace, declared_extension_columns,
+                     fill_lookup_multiplicities)
 
 P = E.P
 _R = 2**64
@@ -298,10 +299,14 @@ class ShardedProver(GpuProver):
                   "composition_trace_commitment", "deep_composition", "fri", "proof_of_work", "queries"]
         torch.cuda.nvtx.range_push("prove:" + phases[0])
 
-        def lap(name):
+        def lap(name, since=None):
             nonlocal t0
             ctx.sync()
             t = time.perf_counter()
+            if since is not None:           # lookup_multiplicities: timed on its own, outside the phase it runs in
+                timings[name] = t - since
+                t0 += t - since
+                return
             timings[name] = t - t0
             t0 = t
             torch.cuda.nvtx.range_pop()
@@ -319,11 +324,13 @@ class ShardedProver(GpuProver):
             air0.composition_program()
             air0.deep_program()
             air0.extension_program()
+            air0.lookup_programs()
             block_program(air0)              # the composition evaluated block by block
             air0.num_challenges(), air0.num_composition_constraint_coeffs(), air0.trace_arguments()
             self._airs[key] = air0
         air = copy.copy(self._airs[key])
         air.public_inputs = stark.get_public_inputs()
+        check_lookup_trace(air, trace)
         channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
         fq = FP if cfg.FQ_IS_FP else FQ3
         log_n = air.log_n
@@ -343,7 +350,12 @@ class ShardedProver(GpuProver):
             raise ProvingError(f"expected {nbase} base columns of {n} rows")
         needs_full_base = next_ > 0          # extension columns are built from the whole base trace (on every rank)
         if needs_full_base or nbase < G or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
-            base = self._to_device(host_base)
+            base = self._own_copy(host_base) if air.lookups else self._to_device(host_base)
+            if air.lookups:         # every rank fills its own copy (a lookup always has an extension column)
+                ctx.sync()
+                t = time.perf_counter()
+                fill_lookup_multiplicities(ctx, air, base)
+                lap("lookup_multiplicities", since=t)
             base_polys = self._interpolate(base, FP, nbase, log_n)
         else:
             base = None
