@@ -299,7 +299,7 @@ def _gib(b):
 
 
 class _Run:
-    """per-proof state shared by the phases of both residencies"""
+    """per-proof state shared by the phases of every driver (resident, streamed, sharded)"""
 
     def __init__(self, **kw):
         self.__dict__.update(kw)
@@ -429,13 +429,32 @@ class GpuProver:
         """default_prove.  validate=True: stark.validate_constraints checks the trace against the AIR once the extension
         trace is committed, and raises before anything after that commitment is computed; its time is recorded as
         timings["validate_constraints"].  The proof bytes do not depend on it.  (ShardedProver, whose ranks may not hold
-        the whole base trace, does not take it.)"""
+        the whole base trace, refuses it with a ProvingError.)"""
         with torch.cuda.stream(self.stream):
             if validate:
                 return self._prove(stark, options, witness, validate=True)
             return self._prove(stark, options, witness)
 
     def _prove(self, stark, options, witness, validate=False):
+        r = self._start(stark, options, witness, validate)
+        est = peak_bytes(r.n, r.beta, r.nbase, r.next_, r.fq, r.air.ce_blowup_factor, options.fri_folding_factor)
+        if self.pinned_bytes > (self.host_memory_budget or 0):
+            self.release_host_memory()          # heaps pinned under a larger budget are not held past a lower one
+        residency = self.choose_residency(est)
+        self.last_residency = residency
+        r.lap("init_air")
+        if residency == "resident":
+            return self._prove_resident(r)
+        if residency == "streamed_host":
+            # tree t's node heap: beta local heaps of n digests (base, extension if any, composition)
+            r.host_heaps = self._host_heaps(est["host"])[:est["host"]].reshape(-1, r.beta, r.n, 32)
+            r.lap("pin_host_memory")
+        return self._prove_streamed(r)
+
+    def _start(self, stark, options, witness, validate):
+        """the set-up every driver shares: the trace, the cached Air with its compiled programs, this proof's public
+        inputs, the shapes, the channel and the phase clock (r.lap).  Returns the _Run with the phase "init_air" open; the
+        trace's columns are not read yet."""
         ctx = self.ctx
         cfg = stark.AirConfig
         timings = {}
@@ -484,34 +503,26 @@ class GpuProver:
         beta = options.lde_blowup_factor
         log_b = beta.bit_length() - 1
         nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
-        est = peak_bytes(n, beta, nbase, next_, fq, air.ce_blowup_factor, options.fri_folding_factor)
-        if self.pinned_bytes > (self.host_memory_budget or 0):
-            self.release_host_memory()          # heaps pinned under a larger budget are not held past a lower one
-        residency = self.choose_residency(est)
-        self.last_residency = residency
         channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
-        r = _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
-                 beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
-                 timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate, host_heaps=None)
-        lap("init_air")
-        if residency == "resident":
-            return self._prove_resident(r)
-        if residency == "streamed_host":
-            # tree t's node heap: beta local heaps of n digests (base, extension if any, composition)
-            r.host_heaps = self._host_heaps(est["host"])[:est["host"]].reshape(-1, beta, n, 32)
-            lap("pin_host_memory")
-        return self._prove_streamed(r)
+        return _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
+                    beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
+                    timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate, host_heaps=None)
+
+    def _base_columns(self, r):
+        """the trace's base columns, refused unless they are (NUM_BASE_COLUMNS, n)"""
+        base = r.trace.base_columns()
+        if tuple(base.shape) != (r.nbase, r.n):
+            raise ProvingError(f"expected {r.nbase} base columns of {r.n} rows")
+        return base
 
     def _prove_resident(self, r):
-        ctx, stark, trace, air, channel, lap = r.ctx, r.stark, r.trace, r.air, r.channel, r.lap
+        ctx, air, channel, lap = r.ctx, r.air, r.channel, r.lap
         fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
 
         # ---- base trace commitment (prover.rs:46-55).  A host trace is uploaded in column chunks on a second stream
         # while the previous chunk is interpolated and extended (columns are independent until the row hash); a
         # pinned trace — the analogue of the reference's GpuAllocator-backed columns — makes the copies asynchronous.
-        host_base = trace.base_columns()
-        if tuple(host_base.shape) != (nbase, n):
-            raise ProvingError(f"expected {nbase} base columns of {n} rows")
+        host_base = self._base_columns(r)
         if air.lookups:
             # the multiplicities are filled before the commitment, so the upload cannot overlap the transforms here
             base = self._lookup_base(r, host_base)
@@ -663,14 +674,12 @@ class GpuProver:
         return rows[:k], MerkleView(path_nodes, digests[:len(init)], digests[len(init):], N.bit_length() - 1)
 
     def _prove_streamed(self, r):
-        ctx, stark, trace, air, channel, lap = r.ctx, r.stark, r.trace, r.air, r.channel, r.lap
+        ctx, air, channel, lap = r.ctx, r.air, r.channel, r.lap
         fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
         offsets = coset_offsets(log_n, log_b)
 
         # ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
-        host_base = trace.base_columns()
-        if tuple(host_base.shape) != (nbase, n):
-            raise ProvingError(f"expected {nbase} base columns of {n} rows")
+        host_base = self._base_columns(r)
         base = self._lookup_base(r, host_base) if air.lookups else self._to_device(host_base)
         del host_base                           # held no longer than `base`: see release_base_columns below
         base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
@@ -761,7 +770,7 @@ class GpuProver:
                           base_view, ext_view, comp_view)
         return self._finish(r, fri_proof, queries)
 
-    # ---- phases both residencies share
+    # ---- phases every driver shares (ShardedProver included)
     def _lookup_base(self, r, host_base):
         """the prover's own device copy of the base columns (the caller's trace, host or device, is never written) with
         every lookup's multiplicity column filled; timed as timings["lookup_multiplicities"]"""
@@ -856,22 +865,34 @@ class GpuProver:
 
     def _fri(self, r, deep_lde):
         """FRI layers (fri.rs:179-249), the remainder and the proof of work; returns the committed layers"""
-        ctx, channel, options, fq, beta = r.ctx, r.channel, r.options, r.fq, r.beta
-        ff = options.fri_folding_factor
-        log_ff = ff.bit_length() - 1
+        log_ff = r.options.fri_folding_factor.bit_length() - 1
         layers = []
         cur, ln = deep_lde, r.log_N
-        for _ in range(options.fri_num_layers(r.N)):
-            nrows = 1 << (ln - log_ff)
-            leaves, nodes = self._empty(nrows, 4), self._empty(nrows, 4)
-            root = ctx.merkle_commit_rows(cur, ff * fq, nrows, leaves=leaves, nodes=nodes)   # Matrix::from_arrays + from_matrix
-            channel.commit_fri_layer(root)
-            layers.append((cur, _Tree(leaves, nodes, nrows), root, nrows))
-            alpha = channel.draw_fri_alpha()
-            nxt = self._empty(nrows * fq)
-            ctx.fri_fold(cur, nxt, fq, ln, log_ff, np.array([_mont(c) for c in _lift(alpha)], dtype=np.uint64))   # apply_drp, offset ONE
-            cur, ln = nxt, ln - log_ff
-        # set_remainder (fri.rs:233-249)
+        for _ in range(r.options.fri_num_layers(r.N)):
+            layer, cur = self._fri_layer(r, cur, ln)
+            layers.append(layer)
+            ln -= log_ff
+        self._fri_tail(r, cur, ln)
+        return layers
+
+    def _fri_layer(self, r, cur, ln):
+        """one FRI layer of the whole codeword `cur` (2^ln entries): commit its rows of ff entries, draw alpha, fold.
+        Returns the layer (evals, tree, root, rows) and the folded codeword."""
+        ctx, channel, fq = r.ctx, r.channel, r.fq
+        ff = r.options.fri_folding_factor
+        log_ff = ff.bit_length() - 1
+        nrows = 1 << (ln - log_ff)
+        leaves, nodes = self._empty(nrows, 4), self._empty(nrows, 4)
+        root = ctx.merkle_commit_rows(cur, ff * fq, nrows, leaves=leaves, nodes=nodes)   # Matrix::from_arrays + from_matrix
+        channel.commit_fri_layer(root)
+        alpha = channel.draw_fri_alpha()
+        nxt = self._empty(nrows * fq)
+        ctx.fri_fold(cur, nxt, fq, ln, log_ff, np.array([_mont(c) for c in _lift(alpha)], dtype=np.uint64))   # apply_drp, offset ONE
+        return (cur, _Tree(leaves, nodes, nrows), root, nrows), nxt
+
+    def _fri_tail(self, r, cur, ln):
+        """set_remainder (fri.rs:233-249) from the last folded codeword `cur` (2^ln entries), then the proof of work"""
+        ctx, channel, options, fq, beta = r.ctx, r.channel, r.options, r.fq, r.beta
         rem_size = 1 << ln
         if rem_size > options.fri_max_remainder_coeffs * beta:
             raise ProvingError("remainder domain too large")
@@ -889,7 +910,6 @@ class GpuProver:
 
         channel.grind_fri_commitments()
         r.lap("proof_of_work")
-        return layers
 
     def _fri_queries(self, r, layers, positions):
         """FRI layer rows and paths at the folded query positions (fri.rs:151-177)"""

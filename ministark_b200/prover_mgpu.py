@@ -22,26 +22,27 @@ proof bytes are identical to the single-GPU prover's (tests/test_gpu_multi.py), 
 
 A FRI layer is sharded while every rank still holds at least two of its rows; the remaining small layers are gathered
 once and finished on every rank.  torch / torch.distributed are plumbing: buffers, the stream, the collectives.
+
+ShardedProver is a GpuProver: only what depends on where the LDE rows live is written here (the column-split
+interpolation, the slab LDE and commitment, the block-wise constraint evaluation and DEEP, the sharded FRI layers and
+the query fetch plan).  The set-up, the phase clock, the base-column read, the lookup fill, the extension and
+composition columns, the OOD/DEEP binding, the gathered FRI layers, the remainder and proof of work, and the proof
+assembly are GpuProver's methods, shared with its resident and streamed drivers.
 """
 import hashlib
-import time
 
 import numpy as np
 import torch
 
-from . import FP, FQ3, GENERATOR as GEN_MONT, ONE
-from . import deep
+from . import FP, GENERATOR as GEN_MONT
 from . import expr as E
 from .air import domain_generator
-from .channel import ProverChannel
 from .cosets import block_program, brev as _brev, coset_offsets, merkle_walk
-from .proof import FriProof, LayerProof, MerkleView, Proof, Queries
-from .prover import (GpuProver, ProvingError, _Tree, _canon_rows, _lift, _mont, check_lookup_trace, declared_extension_columns,
-                     fill_lookup_multiplicities)
+from .proof import LayerProof, MerkleView, Queries
+from .prover import GpuProver, ProvingError, _Run, _canon_rows, _lift, _mont
 
 P = E.P
 _R = 2**64
-_RINV = pow(_R, -1, P)
 
 
 def top_levels(sub_roots):
@@ -246,12 +247,14 @@ class ShardedProver(GpuProver):
         """FriProver::build_layers (src/fri.rs:199-231) on a codeword sharded by rows: `slab` holds this rank's
         2^log_n / G consecutive entries of the bit-reversed codeword.  Per layer: rows of ff entries -> leaf hashes ->
         subtree -> all-gather of the G subtree roots -> channel; the fold is local (row k needs only row k).  Layers with
-        fewer than 2 rows per rank are gathered once and finished on every rank.  Returns (layers, remainder codeword
-        (replicated), its log size); layers = [(evals, tree, root, rows in the layer, sharded?)]."""
+        fewer than 2 rows per rank are gathered once and finished on every rank by GpuProver._fri_layer.  Returns (sharded
+        layers, gathered layers, last folded codeword (replicated), its log size); a layer is (evals, tree, root, rows in
+        the layer), the tree of a sharded layer a _ShardedTree."""
         ctx, dist, G, rank = self.ctx, self.dist, self.world, self.rank
         ff = options.fri_folding_factor
         log_ff = ff.bit_length() - 1
-        layers = []
+        run = _Run(ctx=ctx, channel=channel, fq=fq, options=options)        # what _fri_layer reads
+        layers, gathered = [], []
         cur, ln, sharded = slab, log_n, True
         for _ in range(options.fri_num_layers(1 << log_n)):
             nrows = 1 << (ln - log_ff)
@@ -265,101 +268,48 @@ class ShardedProver(GpuProver):
                 sub = ctx.merkle_commit_rows(cur, ff * fq, nloc, leaves=leaves, nodes=nodes)
                 tree, root = self._finish_tree(sub, leaves, nodes, nloc)
                 channel.commit_fri_layer(root)
-                layers.append((cur, tree, root, nrows, True))
+                layers.append((cur, tree, root, nrows))
                 alpha = channel.draw_fri_alpha()
                 nxt = self._empty(nloc * fq)
                 off = pow(domain_generator(ln), _brev(rank, self.log_g), P) * _R % P      # ONE * g_(2^ln)^bitrev(rank)
                 ctx.fri_fold(cur, nxt, fq, ln - self.log_g, log_ff,
                              np.array([_mont(c) for c in _lift(alpha)], dtype=np.uint64), offset=off)
             else:
-                leaves, nodes = self._empty(nrows, 4), self._empty(nrows, 4)
-                root = ctx.merkle_commit_rows(cur, ff * fq, nrows, leaves=leaves, nodes=nodes)
-                channel.commit_fri_layer(root)
-                layers.append((cur, _Tree(leaves, nodes, nrows), root, nrows, False))
-                alpha = channel.draw_fri_alpha()
-                nxt = self._empty(nrows * fq)
-                ctx.fri_fold(cur, nxt, fq, ln, log_ff, np.array([_mont(c) for c in _lift(alpha)], dtype=np.uint64))
+                layer, nxt = self._fri_layer(run, cur, ln)
+                gathered.append(layer)
             cur, ln = nxt, ln - log_ff
         if sharded:
             full = self._empty((1 << ln) * fq)
             dist.all_gather_into_tensor(full, cur)
             cur = full
-        return layers, cur, ln
+        return layers, gathered, cur, ln
 
-    # ---- default_prove
-    def _prove(self, stark, options, witness):
-        ctx, dist, G, rank = self.ctx, self.dist, self.world, self.rank
-        cfg = stark.AirConfig
-        timings = {}
-        t_all = t0 = time.perf_counter()
-
-        # NVTX range per prover phase (visible to nsys / ncu --nvtx): the range of phase k is closed and the range of
-        # phase k + 1 opened where the reference prints its per-phase timings (src/prover.rs:40-170)
-        phases = ["init_air", "base_trace_commitment", "extension_trace_commitment", "constraint_eval",
-                  "composition_trace_commitment", "deep_composition", "fri", "proof_of_work", "queries"]
-        torch.cuda.nvtx.range_push("prove:" + phases[0])
-
-        def lap(name, since=None):
-            nonlocal t0
-            ctx.sync()
-            t = time.perf_counter()
-            if since is not None:           # lookup_multiplicities: timed on its own, outside the phase it runs in
-                timings[name] = t - since
-                t0 += t - since
-                return
-            timings[name] = t - t0
-            t0 = t
-            torch.cuda.nvtx.range_pop()
-            k = phases.index(name) + 1
-            if k < len(phases):
-                torch.cuda.nvtx.range_push("prove:" + phases[k])
-
-        import copy
-        from .air import Air
-        trace = stark.generate_trace(witness)
-        n = len(trace)
-        key = (cfg, n, options)
-        if key not in self._airs:
-            air0 = Air(cfg, n, None, options)
-            air0.composition_program()
-            air0.deep_program()
-            air0.extension_program()
-            air0.lookup_programs()
-            block_program(air0)              # the composition evaluated block by block
-            air0.num_challenges(), air0.num_composition_constraint_coeffs(), air0.trace_arguments()
-            self._airs[key] = air0
-        air = copy.copy(self._airs[key])
-        air.public_inputs = stark.get_public_inputs()
-        check_lookup_trace(air, trace)
-        channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
-        fq = FP if cfg.FQ_IS_FP else FQ3
-        log_n = air.log_n
-        beta = options.lde_blowup_factor
-        log_b = beta.bit_length() - 1
-        log_N, N = log_n + log_b, n * beta
-        if beta % G or n < 16:
+    # ---- default_prove: the set-up and every phase that does not depend on where the LDE rows live are GpuProver's
+    def _prove(self, stark, options, witness, validate=False):
+        if validate:
+            raise ProvingError("the sharded prover does not validate the trace (its ranks need not hold the whole base "
+                               "trace): validate with GpuProver")
+        r = self._start(stark, options, witness, False)
+        ctx, dist, G = self.ctx, self.dist, self.world
+        air, channel, lap = r.air, r.channel, r.lap
+        fq, n, log_n, log_b, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.nbase, r.next_
+        if r.beta % G or n < 16:
             raise ProvingError("the sharded prover needs a world size dividing the LDE blow-up factor and n >= 16")
-        bpr, rows_per = beta // G, N // G
+        bpr, rows_per = r.beta // G, r.N // G
         my_blocks = self._offsets(log_n, log_b)
-        nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
         lap("init_air")
 
         # ---- base trace commitment (prover.rs:46-55)
-        host_base = trace.base_columns()
-        if tuple(host_base.shape) != (nbase, n):
-            raise ProvingError(f"expected {nbase} base columns of {n} rows")
+        host_base = self._base_columns(r)
         needs_full_base = next_ > 0          # extension columns are built from the whole base trace (on every rank)
         if needs_full_base or nbase < G or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
-            base = self._own_copy(host_base) if air.lookups else self._to_device(host_base)
-            if air.lookups:         # every rank fills its own copy (a lookup always has an extension column)
-                ctx.sync()
-                t = time.perf_counter()
-                fill_lookup_multiplicities(ctx, air, base)
-                lap("lookup_multiplicities", since=t)
+            # with lookups every rank fills its own copy (a lookup always has an extension column)
+            base = self._lookup_base(r, host_base) if air.lookups else self._to_device(host_base)
             base_polys = self._interpolate(base, FP, nbase, log_n)
         else:
             base = None
             base_polys = self._interpolate(host_base, FP, nbase, log_n, from_host=True)
+        del host_base
         base_slab = self._lde_slab(base_polys, FP, nbase, log_n, log_b)
         base_tree, base_root = self._commit_slab(base_slab, FP, nbase, rows_per)
         channel.commit_base_trace(base_root)
@@ -367,18 +317,9 @@ class ShardedProver(GpuProver):
         challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
         hints = air.gen_hints(challenges)
 
-        # ---- extension trace commitment (prover.rs:56-72): built from the (replicated) base trace on every rank, by the
-        # trace's own builder or, without one, from the AIR's declaration
-        if hasattr(trace, "build_extension_columns_device"):
-            ext = trace.build_extension_columns_device(challenges, ctx, base)
-        else:
-            ext = trace.build_extension_columns(challenges)
-            if ext is None and air.extension_declaration:
-                ext = declared_extension_columns(ctx, air, challenges, hints, base, self.device)
+        # ---- extension trace commitment (prover.rs:56-72): built from the (replicated) base trace on every rank
+        ext = self._extension_columns(r, challenges, hints, base)
         del base
-        num_ext = 0 if ext is None else int(ext.shape[0])
-        if num_ext != next_:
-            raise ProvingError(f"expected {next_} extension columns, got {num_ext}")
         ext_polys = ext_slab = ext_tree = None
         if ext is not None:
             ext_polys = self._interpolate(self._to_device(ext), fq, next_, log_n)
@@ -394,7 +335,7 @@ class ShardedProver(GpuProver):
         log_ce = log_n + ce_blowup.bit_length() - 1
         M = n * ce_blowup
         composition_coeffs = [channel.public_coin.draw() for _ in range(air.num_composition_constraint_coeffs())]
-        prog = air._block_program.bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
+        prog = block_program(r.cached_air).bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
         comp_evals = self._empty(M * fq)
         is_fq = [False] * nbase + [True] * next_
         for j, (q, h) in enumerate(my_blocks):
@@ -412,54 +353,15 @@ class ShardedProver(GpuProver):
         # comp_evals is the bit-reversed ce-domain column; one small transform, done on every rank
         ctx.bit_reverse(comp_evals, fq, log_ce)
         ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
-        if ce_blowup == 1:
-            comp_polys = comp_evals.view(1, n * fq)
-        else:
-            comp_polys = self._empty(ce_blowup, n * fq)
-            ctx.matrix_from_rows(comp_evals, comp_polys, fq, n, ce_blowup)
+        comp_polys = self._composition_columns(r, comp_evals)
         comp_slab = self._lde_slab(comp_polys, fq, ce_blowup, log_n, log_b)
         comp_tree, comp_root = self._commit_slab(comp_slab, fq, ce_blowup, rows_per)
         channel.commit_composition_trace(comp_root)
         lap("composition_trace_commitment")
 
-        # ---- out-of-domain evaluations (composer.rs:43-86) from the replicated coefficients
-        z = channel.get_ood_point()
-        zq = _lift(z)
-        trace_arguments = air.trace_arguments()
-        offsets = sorted(set(o for _, o in trace_arguments))
-        z_points, z_m = deep.ood_points(zq, log_n, offsets, ce_blowup)
-        pts = np.array([[_mont(c) for c in z_points[o]] for o in offsets], dtype=np.uint64).reshape(-1, 3)
-        base_ood = ctx.poly_eval(base_polys, FP, n, nbase, pts)
-        ext_ood = ctx.poly_eval(ext_polys, fq, n, next_, pts) if next_ else None
-        comp_ood = ctx.poly_eval(comp_polys, fq, n, ce_blowup, np.array([[_mont(c) for c in z_m]], dtype=np.uint64))
-
-        def unlift(w3):
-            t = tuple(int(w) * _RINV % P for w in w3)
-            if fq == FP:
-                if t[1] or t[2]:
-                    raise ProvingError("out-of-domain value left the base field although Fq = Fp")
-                return t[0]
-            return t
-
-        execution_trace_oods = []
-        for col, off in trace_arguments:
-            k = offsets.index(off)
-            if col < nbase:
-                execution_trace_oods.append(unlift(base_ood[col, k]))
-            elif col < nbase + next_:
-                execution_trace_oods.append(unlift(ext_ood[col - nbase, k]))
-            else:
-                raise ProvingError(f"column is {col} but there are only {nbase + next_} columns")
-        composition_trace_oods = [unlift(comp_ood[j, 0]) for j in range(ce_blowup)]
-        channel.send_ood_evals(execution_trace_oods, composition_trace_oods)
-
-        # ---- DEEP composition polynomial over this rank's LDE rows (composer.rs:89-188 in evaluation form)
-        ex_alphas, co_alphas, (d_alpha, d_beta) = stark.gen_deep_coeffs(channel.public_coin, air)
-        dprog_sym, dkeys = air.deep_program()
-        dprog = dprog_sym.bind(hints=deep.deep_hint_values(
-            dkeys, z_points, z_m, [_lift(v) for v in execution_trace_oods], [_lift(v) for v in composition_trace_oods],
-            [_lift(v) for v in ex_alphas], [_lift(v) for v in co_alphas], _lift(d_alpha), _lift(d_beta),
-            trace_arguments=trace_arguments))
+        # ---- DEEP composition polynomial over this rank's LDE rows (composer.rs:89-188 in evaluation form), bound from
+        # the out-of-domain evaluations of the replicated coefficients
+        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
         ncols_all = nbase + next_ + ce_blowup
         deep_slab = self._empty(rows_per * fq)
         for j, (q, h) in enumerate(my_blocks):
@@ -473,40 +375,20 @@ class ShardedProver(GpuProver):
         lap("deep_composition")
 
         # ---- FRI (fri.rs:179-249): layers sharded by rows while every rank keeps >= 2 rows of the layer
-        layers, cur, ln = self.fri_commit(deep_slab, log_N, fq, options, channel)
-        ff = options.fri_folding_factor
-        rem_size = 1 << ln
-        if rem_size > options.fri_max_remainder_coeffs * beta:
-            raise ProvingError("remainder domain too large")
-        rem = cur.clone()
-        ctx.bit_reverse(rem, fq, ln)
-        ctx.ntt_batch(rem, fq, ln, 1, inverse=True, offset=ONE)
-        ctx.sync()
-        rem_coeffs = _canon_rows(rem.cpu().numpy().view(np.uint64), fq)
-        keep = rem_size // beta
-        zero = 0 if fq == FP else (0, 0, 0)
-        if any(c != zero for c in rem_coeffs[keep:]):
-            raise ProvingError("FRI remainder is not low degree: the trace does not satisfy the AIR (fri.rs:246)")
-        channel.commit_remainder(rem_coeffs[:keep])
-        lap("fri")
-
-        channel.grind_fri_commitments()
-        lap("proof_of_work")
+        layers, gathered, cur, ln = self.fri_commit(deep_slab, r.log_N, fq, options, channel)
+        self._fri_tail(r, cur, ln)
 
         # ---- queries (fri.rs:151-177, trace.rs:115-157): rows and path digests come from the ranks that own them
+        ff = options.fri_folding_factor
         positions = channel.get_fri_query_positions()
         pos_sorted = sorted(set(positions))
         plan = _FetchPlan(self)
         pending, folded = [], positions
-        for evals, tree, root, nrows, was_sharded in layers:
+        for evals, tree, root, nrows in layers:
             folded = sorted(set(p // ff for p in folded))
-            if was_sharded:
-                nloc = nrows // G
-                hr = plan.rows(lambda loc, e=evals, k=nloc: ctx.gather_rows_rowmajor(e, ff * fq, k, loc), nloc, folded, ff * fq)
-                pending.append((root, hr, plan.view(tree, folded), None))
-            else:
-                rows = ctx.gather_rows_rowmajor(evals, ff * fq, nrows, folded)
-                pending.append((root, None, None, (rows, self._view(tree, folded))))
+            nloc = nrows // G
+            hr = plan.rows(lambda loc, e=evals, k=nloc: ctx.gather_rows_rowmajor(e, ff * fq, k, loc), nloc, folded, ff * fq)
+            pending.append((root, hr, plan.view(tree, folded)))
 
         def trace_rows(slab, field, ncols):
             # Queries::new keeps the caller's position order (sorted, deduplicated by draw_queries)
@@ -518,18 +400,11 @@ class ShardedProver(GpuProver):
         v_base, v_comp = plan.view(base_tree, pos_sorted), plan.view(comp_tree, pos_sorted)
         v_ext = plan.view(ext_tree, pos_sorted) if next_ else None
         plan.execute()
-        fri_layers = []
-        for root, hr, hv, direct in pending:
-            rows, view = (plan.get_rows(hr), plan.get_view(hv)) if direct is None else direct
-            fri_layers.append(LayerProof(_canon_rows(rows, fq), view, root))
-        fri_proof = FriProof(fri_layers, channel.fri_remainder_coeffs)
+        fri_proof = self._fri_queries(r, gathered, folded)      # the gathered layers: on every rank
+        fri_proof.layers[:0] = [LayerProof(_canon_rows(plan.get_rows(hr), fq), plan.get_view(hv), root) for root, hr, hv in pending]
         queries = Queries(
             _canon_rows(plan.get_rows(h_base), 1),
             _canon_rows(plan.get_rows(h_ext), fq) if next_ else [],
             _canon_rows(plan.get_rows(h_comp), fq),
             plan.get_view(v_base), plan.get_view(v_ext) if next_ else None, plan.get_view(v_comp))
-        lap("queries")
-        timings["total"] = time.perf_counter() - t_all
-        return Proof(options, n, channel.base_trace_commitment, channel.extension_trace_commitment,
-                     channel.composition_trace_commitment, fri_proof, channel.pow_nonce, queries,
-                     channel.execution_trace_ood_evals, channel.composition_trace_ood_evals, timings)
+        return self._finish(r, fri_proof, queries)

@@ -4,8 +4,8 @@ oracle's build of the C ABI underneath `ministark_b200._lib`, host tensors, no-o
   * `GpuProver` (ministark_b200/prover.py): proof bytes == oracle/stark_oracle.cpu_prove for examples/fib, the Fq3
     permutation AIR and examples/brainfuck (extension columns through `build_extension_columns_device`);
   * `ShardedProver` (ministark_b200/prover_mgpu.py) over gloo, world size 2 and 4: every matrix sharded by LDE coset
-    blocks, FRI layers by rows, Merkle paths assembled from their owners — the bytes must equal the single prover's.
-    This is the CPU cover of the N > 1 prover path (the NCCL run of the same code is tests/test_gpu_multi.py).
+    blocks, FRI layers by rows, Merkle paths assembled from their owners — the bytes must equal the single prover's;
+    `validate=True` is refused before the trace is read.  This is the CPU cover of the N > 1 prover path (the NCCL run of the same code is tests/test_gpu_multi.py).
 Every multi-process case runs in spawned workers that install the harness themselves; the pytest process never does."""
 import os
 import socket
@@ -87,7 +87,22 @@ def _sharded_worker(rank, world, port, which, q):
         claim, opts, trace = _make_case(which)
         prover = ShardedProver(dist, rank)
         first = prover.prove(claim, ProofOptions(*opts), trace).to_bytes()
-        q.put((rank, first, prover.prove(claim, ProofOptions(*opts), trace).to_bytes()))
+        second = prover.prove(claim, ProofOptions(*opts), trace).to_bytes()
+
+        class Unread:
+            """a witness whose columns must not be read: validate=True is refused before any work"""
+            def __len__(self):
+                return len(trace)
+
+            def base_columns(self):
+                raise AssertionError("the base columns were read")
+
+        try:
+            prover.prove(claim, ProofOptions(*opts), Unread(), validate=True)
+            refusal = None
+        except Exception as e:
+            refusal = f"{type(e).__name__}: {e}"
+        q.put((rank, first, second, refusal))
     finally:
         dist.destroy_process_group()
 
@@ -110,8 +125,9 @@ def test_sharded_prover_over_gloo_bytes_equal_cpu_restatement(orc, world, which)
         p.join(timeout=120)
         assert p.exitcode == 0
     want = _cpu_restatement(which)
-    for rank, first, second in got:                 # every rank assembles the same proof, twice
+    for rank, first, second, refusal in got:        # every rank assembles the same proof, twice
         assert first == second == want, f"rank {rank}"
+        assert refusal and refusal.startswith("ProvingError: ") and "sharded prover does not validate" in refusal, refusal
 
 
 def _bad_input_worker(q):
