@@ -397,6 +397,15 @@ class Context:
         """the eight helper columns of BrainfuckTrace.helper_columns() from a (17, n) base matrix into (8, n) `aux`"""
         self._ck(self.lib.ms_bf_helper_columns(self.h, _ptr(base), n, _ptr(aux)))
 
+    # ---- examples/rescue trace (include/ministark_rescue.h)
+    def rescue_chains(self, seed, K, L, out):
+        """write `out`, the (12, 8 K L) matrix of K chains of L Rescue-Prime permutations from the four canonical seed
+        words (ms_rescue_chains); not synchronised"""
+        s = np.array([int(v) for v in seed], dtype=np.uint64)
+        if s.size != 4:
+            raise MsError("ms_rescue_chains: the seed is four words")
+        self._ck(self.lib.ms_rescue_chains(self.h, s.ctypes.data, int(K), int(L), _ptr(out)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

@@ -17,6 +17,7 @@ LOOKUP_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
+RESCUE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -111,6 +112,11 @@ _HOST_NODES_SIGS = {
     "ms_merkle_commit_block_sha256_host": (ci, [vp, ci, vp, sz, ui, ui, vp, vp]),
 }
 
+# include/ministark_rescue.h: the trace of examples/rescue (Rescue-Prime permutation chains) built on the device
+_RESCUE_SIGS = {
+    "ms_rescue_chains": (ci, [vp, vp, u64, u64, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -145,6 +151,7 @@ def load():
         bind(lib, _BF_SIGS)
         bind(lib, _DEVICE_SIGS)
         bind(lib, _HOST_NODES_SIGS)
+        bind(lib, _RESCUE_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

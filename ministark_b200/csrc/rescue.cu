@@ -1,0 +1,129 @@
+// rescue.cu — the trace of examples/rescue (include/ministark_rescue.h): K independent chains of L Rescue-Prime
+// permutations, side by side on the device.
+//
+// One chain per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's parameters and
+// write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the MDS product is
+// 12 shuffles and 12 multiply-adds per lane.  The S-box is x^7 (4 multiplications), the inverse S-box x^(1/7) a fixed
+// addition chain of 63 squarings and 9 multiplications.  A chain is one long dependent sequence (7 L rounds of about
+// 100 field multiplications each), so the kernel is bound by the latency of that sequence, not by HBM: 12 n words are
+// written in all, each lane storing its own column's rows in order.
+#include "../../include/ministark_rescue.h"
+#include "ctx.cuh"
+#include "rescue_params.cuh"
+
+namespace ms {
+
+constexpr int kW = MS_RESCUE_WIDTH, kRounds = MS_RESCUE_ROUNDS;
+constexpr unsigned kLanes = 16;         // lanes per chain
+constexpr unsigned kThreads = 128;      // 8 chains per block
+
+static __constant__ u64 kRc[2 * kW * kRounds] = MS_RESCUE_RC;      // canonical words
+static __constant__ u64 kMds[kW * kW] = MS_RESCUE_MDS;
+
+// the exponent the chain of inv_sbox computes: e3 = 0b100100 = 36, e4 = e3 * 2^6 + e3, e5 = e4 * 2^12 + e4,
+// e6 = e5 * 2^6 + e3, e7 = e6 * 2^31 + e6, then ((e7 * 2 + e6) * 4) + 7
+constexpr u64 chain_exponent() {
+    const u64 e3 = 36, e4 = (e3 << 6) + e3, e5 = (e4 << 12) + e4, e6 = (e5 << 6) + e3, e7 = (e6 << 31) + e6;
+    return (((e7 << 1) + e6) << 2) + 7;
+}
+static_assert(chain_exponent() == MS_RESCUE_ALPHA_INV, "the inverse S-box chain must compute x^(1/7)");
+
+template <int K>
+__device__ __forceinline__ u64 exp_acc(u64 base, u64 tail) {     // base^(2^K) * tail
+#pragma unroll
+    for (int i = 0; i < K; i++) base = gl::sqr(base);
+    return gl::mul(base, tail);
+}
+
+__device__ __forceinline__ u64 inv_sbox(u64 x) {
+    const u64 t1 = gl::sqr(x), t2 = gl::sqr(t1);
+    const u64 t3 = exp_acc<3>(t2, t2);
+    const u64 t4 = exp_acc<6>(t3, t3);
+    const u64 t5 = exp_acc<12>(t4, t4);
+    const u64 t6 = exp_acc<6>(t5, t3);
+    const u64 t7 = exp_acc<31>(t6, t6);
+    const u64 a = gl::sqr(gl::sqr(gl::mul(gl::sqr(t7), t6)));
+    return gl::mul(a, gl::mul(gl::mul(t1, t2), x));
+}
+
+// word `lane` of MDS v, v spread over the chain's 16 lanes one word each
+__device__ __forceinline__ u64 mds_apply(const u64 (&row)[kW], u64 v) {
+    u64 acc = 0;
+#pragma unroll
+    for (int j = 0; j < kW; j++) acc = gl::add(acc, gl::mul(row[j], __shfl_sync(~0u, v, j, kLanes)));
+    return acc;
+}
+
+struct ChainArgs {
+    u64 seed[4];        // Montgomery
+    u64 tag_root;       // Montgomery w_K
+    u64 K, L, n;
+    u64 *out;
+};
+
+__global__ void __launch_bounds__(kThreads) rescue_chains_kernel(ChainArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 chain = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool live = chain < a.K && lane < (unsigned)kW;       // every lane runs: the shuffles take the whole warp
+    const unsigned w = lane < (unsigned)kW ? lane : kW - 1;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+#pragma unroll
+    for (int j = 0; j < kW; j++) row[j] = gl::to_mont(kMds[w * kW + j]);
+#pragma unroll
+    for (int r = 0; r < kRounds; r++) {
+        c1[r] = gl::to_mont(kRc[2 * kW * r + w]);
+        c2[r] = gl::to_mont(kRc[2 * kW * r + kW + w]);
+    }
+    u64 s = 0;
+    if (lane < 4) s = lane == 0 ? a.seed[0] : lane == 1 ? a.seed[1] : lane == 2 ? a.seed[2] : a.seed[3];
+    else if (lane == 4) s = gl::pow(a.tag_root, chain < a.K ? chain : 0);
+    u64 *col = a.out + (u64)w * a.n + (chain < a.K ? chain : 0) * 8 * a.L;
+    for (u64 j = 0; j < a.L; j++, col += 8) {
+#pragma unroll
+        for (int r = 0; r < kRounds; r++) {
+            if (live) col[r] = s;
+            const u64 x3 = gl::mul(gl::sqr(s), s);
+            s = gl::add(mds_apply(row, gl::mul(gl::sqr(x3), s)), c1[r]);
+            s = gl::add(mds_apply(row, inv_sbox(s)), c2[r]);
+        }
+        if (live) col[kRounds] = s;
+    }
+}
+
+static bool pow2(u64 v) { return v && !(v & (v - 1)); }
+static unsigned log2u(u64 v) { return 63 - __builtin_clzll(v); }
+
+}  // namespace ms
+
+using namespace ms;
+
+extern "C" int ms_rescue_chains(ms_ctx *c, const uint64_t *seed, uint64_t K, uint64_t L, void *out) {
+    if (!c) return MS_ERR_INVALID;
+    if (!seed || !out) return fail(c, MS_ERR_INVALID, "ms_rescue_chains: null argument");
+    if (!pow2(K) || !pow2(L))
+        return fail(c, MS_ERR_INVALID, "ms_rescue_chains: K = %llu and L = %llu must be powers of two",
+                    (unsigned long long)K, (unsigned long long)L);
+    if (log2u(K) + log2u(L) + 3 > 32)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_chains: 8 K L rows (K = %llu, L = %llu) exceed 2^32",
+                    (unsigned long long)K, (unsigned long long)L);
+    for (int w = 0; w < 4; w++)
+        if (seed[w] >= gl::P)
+            return fail(c, MS_ERR_INVALID, "ms_rescue_chains: seed word %d (%llu) is not canonical", w, (unsigned long long)seed[w]);
+    const u64 n = 8 * K * L;
+    ChainArgs a;
+    for (int w = 0; w < 4; w++) a.seed[w] = gl::to_mont(seed[w]);
+    // ark-ff's root of unity of order 2^32 (7^((p - 1) / 2^32)), raised to 2^(32 - log2 K)
+    constexpr u64 kTwoAdicRoot = 1753635133440165772ull;
+    a.tag_root = gl::pow(gl::to_mont(kTwoAdicRoot), 1ull << (32 - log2u(K)));
+    a.K = K;
+    a.L = L;
+    a.n = n;
+    Staged O(c, out, (size_t)kW * n * 8, false, true);
+    if (O.rc) return O.rc;
+    a.out = O.as<u64>();
+    const u64 blocks = (K * kLanes + kThreads - 1) / kThreads;
+    rescue_chains_kernel<<<(unsigned)blocks, kThreads, 0, c->stream>>>(a);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    return O.finish();
+}
