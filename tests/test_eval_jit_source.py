@@ -6,7 +6,8 @@ arithmetic, so the very text NVRTC compiles is compiled here by g++ behind a doz
 __ldg, __brevll ...), run for every point of a small domain and compared with the compiled CPU interpreter of the same
 program (oracle/cpu_abi.c, itself checked against the tree-walking oracle in tests/test_cpp_cpu_abi.py).  Programs: the
 composition and DEEP programs of the three example AIRs as the provers build them (grouped DEEP, shared powers, batched
-inversions, leaf rematerialisation), bound to random verifier values, in the storage orders the provers use."""
+inversions, leaf rematerialisation), bound to random verifier values, in the storage orders the provers use; and every
+opcode over every operand-field combination on edge operands, against big integers."""
 import ctypes as C
 import os
 import random
@@ -20,6 +21,8 @@ from ministark_b200 import expr as E
 from ministark_b200.air import Air, ProofOptions
 from ministark_b200.examples import brainfuck as bf
 from ministark_b200.examples import fib, perm
+
+import tests_helpers_expr as H
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P = E.P
@@ -54,7 +57,7 @@ extern "C" void run_all(const u64 *const *col_ptr, const u64 *kc, const u64 *tw_
 """
 
 
-def _host_kernel(tmp, prog, fq):
+def _kernel_source(tmp, prog, fq):
     lib = _lib.load()
     src_path = os.path.join(tmp, "k.cu")
     os.environ["MS_EVAL_JIT_DUMP"] = src_path
@@ -66,8 +69,12 @@ def _host_kernel(tmp, prog, fq):
     if rc == 1:
         pytest.skip("NVRTC is not installed: no specialised kernel is generated")
     assert rc == 0, log.value.decode()[:2000]
+    return open(src_path).read()
+
+
+def _host_kernel(tmp, prog, fq):
     with open(os.path.join(tmp, "k.cpp"), "w") as f:
-        f.write(PRELUDE + open(src_path).read() + DRIVER)
+        f.write(PRELUDE + _kernel_source(tmp, prog, fq) + DRIVER)
     so = os.path.join(tmp, "k.so")
     subprocess.check_call(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-w", "-o", so, os.path.join(tmp, "k.cpp")])
     return C.CDLL(so)
@@ -152,3 +159,40 @@ def test_generated_kernel_source_of_the_config3_program(tmp_path, orc, cpu_abi):
     kernel.run_all(ptrs, C.c_void_p(consts.ctypes.data), C.c_void_p(lo.ctypes.data), C.c_void_p(hi.ctypes.data), C.c_uint(len(hi)),
                    C.c_uint64(GENERATOR), C.c_uint(log_n), 1, 0, C.c_void_p(got.ctypes.data))
     assert np.array_equal(got, synth_oracle.constraint_eval(orc, lde, log_n, log_b, ncols))
+
+
+@pytest.mark.parametrize("fq", [3, 1])
+def test_generated_kernel_source_on_edge_operands(tmp_path, fq):
+    """every opcode over every operand-field combination on edge operands (tests_helpers_expr.edge_programs, the programs
+    tests/test_gpu_eval_edges.py runs on the device): the host branches of the generated source against pyspec's big
+    integers.  All kernels go into one host library, the field code once and each kernel under its own name."""
+    programs = H.edge_programs()
+    kernel_start = 'extern "C" __global__'
+    field_src, kernels, drivers = None, [], []
+    for k, (_, prog, _, _) in enumerate(programs):
+        src = _kernel_source(str(tmp_path), prog, fq)
+        head, sep, body = src.partition(kernel_start)
+        assert sep and (field_src is None or head == field_src)
+        field_src = head
+        kernels.append(sep + body.replace("ms_eval_jit(", f"ms_eval_jit_{k}(", 1))
+        drivers.append(DRIVER.replace("run_all(", f"run_all_{k}(").replace("ms_eval_jit(", f"ms_eval_jit_{k}("))
+    with open(tmp_path / "edges.cpp", "w") as f:
+        f.write(PRELUDE + field_src + "".join(kernels) + "".join(drivers))
+    so = str(tmp_path / "edges.so")
+    subprocess.check_call(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-w", "-o", so, str(tmp_path / "edges.cpp")])
+    lib = C.CDLL(so)
+    log_m = H.EDGE_LOG_M
+    m = 1 << log_m
+    cols, isq = H.edge_columns(fq)
+    words = [np.ascontiguousarray(H.column_words(c, q, fq)) for c, q in zip(cols, isq)]
+    ptrs = (C.c_void_p * len(words))(*[w.ctypes.data for w in words])
+    lo, hi = _tables(log_m)
+    for k, (name, prog, used, ref) in enumerate(programs):
+        want, operands = H.edge_reference(cols, used, ref, fq)
+        got = np.zeros(m * fq, dtype=np.uint64)
+        consts = np.ascontiguousarray(prog.consts)
+        getattr(lib, f"run_all_{k}")(ptrs, C.c_void_p(consts.ctypes.data), C.c_void_p(lo.ctypes.data), C.c_void_p(hi.ctypes.data),
+                                     C.c_uint(len(hi)), C.c_uint64(GENERATOR), C.c_uint(log_m), 0, 0, C.c_void_p(got.ctypes.data))
+        bad = np.nonzero((got.reshape(m, fq) != want.reshape(m, fq)).any(axis=1))[0]
+        assert not len(bad), (f"{name} fq_field={fq}: {len(bad)} points differ, first at {bad[0]} operands {operands(bad[0])}: "
+                              f"got {[hex(w) for w in got.reshape(m, fq)[bad[0]]]}, want {[hex(w) for w in want.reshape(m, fq)[bad[0]]]}")
