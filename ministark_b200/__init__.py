@@ -406,6 +406,12 @@ class Context:
             raise MsError("ms_rescue_chains: the seed is four words")
         self._ck(self.lib.ms_rescue_chains(self.h, s.ctypes.data, int(K), int(L), _ptr(out)))
 
+    # ---- examples/rescue hash trace (include/ministark_rescue_hash.h)
+    def rescue_hash(self, messages, K, length, out):
+        """write `out`, the (13, 8 K L) sponge trace of K messages of `length` canonical words (`messages`: K x length,
+        row-major, host or device; ms_rescue_hash); not synchronised"""
+        self._ck(self.lib.ms_rescue_hash(self.h, _ptr(messages), int(K), int(length), _ptr(out)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

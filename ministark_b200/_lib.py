@@ -18,6 +18,7 @@ BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
 RESCUE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue.h")
+RESCUE_HASH_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_hash.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -117,6 +118,11 @@ _RESCUE_SIGS = {
     "ms_rescue_chains": (ci, [vp, vp, u64, u64, vp]),
 }
 
+# include/ministark_rescue_hash.h: the trace of examples/rescue's hash claim (the Rescue-Prime sponge over K messages)
+_RESCUE_HASH_SIGS = {
+    "ms_rescue_hash": (ci, [vp, vp, u64, u64, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -152,6 +158,7 @@ def load():
         bind(lib, _DEVICE_SIGS)
         bind(lib, _HOST_NODES_SIGS)
         bind(lib, _RESCUE_SIGS)
+        bind(lib, _RESCUE_HASH_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -1,13 +1,16 @@
-// rescue.cu — the trace of examples/rescue (include/ministark_rescue.h): K independent chains of L Rescue-Prime
-// permutations, side by side on the device.
+// rescue.cu — the traces of examples/rescue, side by side on the device: K independent chains of L Rescue-Prime
+// permutations (include/ministark_rescue.h), and K messages absorbed by the Rescue-Prime sponge
+// (include/ministark_rescue_hash.h).
 //
-// One chain per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's parameters and
-// write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the MDS product is
-// 12 shuffles and 12 multiply-adds per lane.  The S-box is x^7 (4 multiplications), the inverse S-box x^(1/7) a fixed
-// addition chain of 63 squarings and 9 multiplications.  A chain is one long dependent sequence (7 L rounds of about
-// 100 field multiplications each), so the kernel is bound by the latency of that sequence, not by HBM: 12 n words are
-// written in all, each lane storing its own column's rows in order.
+// One chain (or message) per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's
+// parameters and write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the
+// MDS product is 12 shuffles and 12 multiply-adds per lane.  The S-box is x^7 (4 multiplications), the inverse S-box
+// x^(1/7) a fixed addition chain of 63 squarings and 9 multiplications.  A chain is one long dependent sequence (7 L
+// rounds of about 100 field multiplications each), so the kernel is bound by the latency of that sequence, not by HBM:
+// 12 n words are written in all (13 n by the hash, whose lanes 0..7 also write the absorbed words), each lane storing
+// its own column's rows in order.  The hash is meant for many short messages: from K = 2^16 on, its grid fills the GPU.
 #include "../../include/ministark_rescue.h"
+#include "../../include/ministark_rescue_hash.h"
 #include "ctx.cuh"
 #include "rescue_params.cuh"
 
@@ -54,6 +57,24 @@ __device__ __forceinline__ u64 mds_apply(const u64 (&row)[kW], u64 v) {
     return acc;
 }
 
+// the lane's MDS row and round constants (Montgomery), word w of the state
+__device__ __forceinline__ void load_params(unsigned w, u64 (&row)[kW], u64 (&c1)[kRounds], u64 (&c2)[kRounds]) {
+#pragma unroll
+    for (int j = 0; j < kW; j++) row[j] = gl::to_mont(kMds[w * kW + j]);
+#pragma unroll
+    for (int r = 0; r < kRounds; r++) {
+        c1[r] = gl::to_mont(kRc[2 * kW * r + w]);
+        c2[r] = gl::to_mont(kRc[2 * kW * r + kW + w]);
+    }
+}
+
+// one round on the chain's 16 lanes: S-box, MDS, the first constants, inverse S-box, MDS, the second constants
+__device__ __forceinline__ u64 rescue_round(const u64 (&row)[kW], u64 c1, u64 c2, u64 s) {
+    const u64 x3 = gl::mul(gl::sqr(s), s);
+    s = gl::add(mds_apply(row, gl::mul(gl::sqr(x3), s)), c1);
+    return gl::add(mds_apply(row, inv_sbox(s)), c2);
+}
+
 struct ChainArgs {
     u64 seed[4];        // Montgomery
     u64 tag_root;       // Montgomery w_K
@@ -67,13 +88,7 @@ __global__ void __launch_bounds__(kThreads) rescue_chains_kernel(ChainArgs a) {
     const bool live = chain < a.K && lane < (unsigned)kW;       // every lane runs: the shuffles take the whole warp
     const unsigned w = lane < (unsigned)kW ? lane : kW - 1;
     u64 row[kW], c1[kRounds], c2[kRounds];
-#pragma unroll
-    for (int j = 0; j < kW; j++) row[j] = gl::to_mont(kMds[w * kW + j]);
-#pragma unroll
-    for (int r = 0; r < kRounds; r++) {
-        c1[r] = gl::to_mont(kRc[2 * kW * r + w]);
-        c2[r] = gl::to_mont(kRc[2 * kW * r + kW + w]);
-    }
+    load_params(w, row, c1, c2);
     u64 s = 0;
     if (lane < 4) s = lane == 0 ? a.seed[0] : lane == 1 ? a.seed[1] : lane == 2 ? a.seed[2] : a.seed[3];
     else if (lane == 4) s = gl::pow(a.tag_root, chain < a.K ? chain : 0);
@@ -82,9 +97,43 @@ __global__ void __launch_bounds__(kThreads) rescue_chains_kernel(ChainArgs a) {
 #pragma unroll
         for (int r = 0; r < kRounds; r++) {
             if (live) col[r] = s;
-            const u64 x3 = gl::mul(gl::sqr(s), s);
-            s = gl::add(mds_apply(row, gl::mul(gl::sqr(x3), s)), c1[r]);
-            s = gl::add(mds_apply(row, inv_sbox(s)), c2[r]);
+            s = rescue_round(row, c1[r], c2[r], s);
+        }
+        if (live) col[kRounds] = s;
+    }
+}
+
+struct HashArgs {
+    const u64 *messages;    // K x length canonical words
+    u64 K, length, L, n;
+    u64 *out;
+};
+
+// the sponge of one message per 16 lanes: before permutation j, lanes 0..7 take word `lane` of block j (a message word,
+// the padding's 1, or 0 in the padding and the filler blocks j >= B), write it to column 12 and add it into the state
+__global__ void __launch_bounds__(kThreads) rescue_hash_kernel(HashArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 msg = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool live = msg < a.K && lane < (unsigned)kW;
+    const unsigned w = lane < (unsigned)kW ? lane : kW - 1;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+    load_params(w, row, c1, c2);
+    const u64 k = msg < a.K ? msg : 0;
+    const u64 *words = a.messages + k * a.length;
+    u64 *col = a.out + (u64)w * a.n + k * 8 * a.L;
+    u64 *mcol = a.out + (u64)kW * a.n + k * 8 * a.L;
+    u64 s = 0;
+    for (u64 j = 0; j < a.L; j++, col += 8, mcol += 8) {
+        if (lane < 8) {
+            const u64 p = 8 * j + lane;
+            const u64 m = p < a.length ? gl::to_mont(words[p]) : p == a.length ? gl::ONE : 0;
+            if (live) mcol[lane] = m;
+            s = gl::add(s, m);
+        }
+#pragma unroll
+        for (int r = 0; r < kRounds; r++) {
+            if (live) col[r] = s;
+            s = rescue_round(row, c1[r], c2[r], s);
         }
         if (live) col[kRounds] = s;
     }
@@ -126,4 +175,34 @@ extern "C" int ms_rescue_chains(ms_ctx *c, const uint64_t *seed, uint64_t K, uin
     c->launches++;
     MS_CHECK_LAUNCH(c);
     return O.finish();
+}
+
+extern "C" int ms_rescue_hash(ms_ctx *c, const uint64_t *messages, uint64_t K, uint64_t length, void *out) {
+    if (!c) return MS_ERR_INVALID;
+    if (!out || (!messages && length)) return fail(c, MS_ERR_INVALID, "ms_rescue_hash: null argument");
+    if (!pow2(K)) return fail(c, MS_ERR_INVALID, "ms_rescue_hash: K = %llu is not a power of two", (unsigned long long)K);
+    const u64 B = length / 8 + 1;                               // the padding always appends its 1
+    const unsigned log_l = B == 1 ? 0 : log2u(B - 1) + 1;       // L = 2^log_l, the smallest power of two >= B
+    if (log2u(K) + log_l + 3 > 32)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_hash: 8 K L rows (K = %llu, length = %llu) exceed 2^32",
+                    (unsigned long long)K, (unsigned long long)length);
+    const u64 L = 1ull << log_l;
+    HashArgs a;
+    a.K = K;
+    a.length = length;
+    a.L = L;
+    a.n = 8 * K * L;
+    Staged O(c, out, (size_t)(kW + 1) * a.n * 8, false, true);
+    if (O.rc) return O.rc;
+    Staged M(c, messages, (size_t)K * length * 8, true, false);
+    if (M.rc) return M.rc;
+    a.out = O.as<u64>();
+    a.messages = M.as<u64>();
+    const u64 blocks = (K * kLanes + kThreads - 1) / kThreads;
+    rescue_hash_kernel<<<(unsigned)blocks, kThreads, 0, c->stream>>>(a);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    const int rc = M.finish();
+    const int rc_out = O.finish();
+    return rc ? rc : rc_out;
 }
