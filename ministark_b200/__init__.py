@@ -366,6 +366,29 @@ class Context:
                  for q in range(ntuples + 1)]
         return pairs[:ntuples], pairs[ntuples]
 
+    def permutation_workspace_bytes(self, log_n, width):
+        """bytes of the workspace permutation_fill needs (ms_permutation_workspace_bytes; arithmetic only)"""
+        out = C.c_size_t()
+        rc = self.lib.ms_permutation_workspace_bytes(log_n, width, C.byref(out))
+        if rc != 0:
+            raise MsError(f"[{rc}] ms_permutation_workspace_bytes: log_n={log_n}, width={width} out of range")
+        return int(out.value)
+
+    def permutation_fill(self, program, targets, log_n, cols, width, workspace):
+        """the target columns of one sorted-copy permutation (include/ministark_permutation.h): `targets`, width device
+        columns of 2^log_n Montgomery words, receive the source tuples of `program` (expr.compile_lookup_program with no
+        value tuples) sorted lexicographically, stably.  `cols`: natural-order base columns (device), then the program's
+        periodic tables; workspace: a device buffer of permutation_workspace_bytes(log_n, width) bytes.  Asynchronous on
+        the context's stream."""
+        k = len(cols)
+        ptrs = (C.c_void_p * max(k, 1))(*[_ptr(c) for c in cols])
+        isq = (C.c_int * max(k, 1))()
+        tgt = (C.c_void_p * max(len(targets), 1))(*[_ptr(t) for t in targets])
+        nbytes = workspace.numel() * workspace.element_size() if hasattr(workspace, "numel") else workspace.nbytes
+        self._ck(self.lib.ms_permutation_fill(self.h, program.code.ctypes.data, len(program), program.consts.ctypes.data,
+                                              program.consts.shape[0], ptrs, isq, k, log_n, width, tgt, _ptr(workspace),
+                                              nbytes))
+
     def poly_eval(self, coeffs, field, n, ncols, points, col_stride=None):
         """horner_evaluate of every column at every point (get_ood_evals, src/composer.rs:43-86).
         points: (k, 3) Montgomery words; returns (ncols, k, 3) numpy uint64."""

@@ -14,6 +14,7 @@ STREAM_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_
 CHECK_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_check.h")
 EXTENSION_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_extension.h")
 LOOKUP_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_lookup.h")
+PERMUTATION_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_permutation.h")
 BF_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_bf.h")
 DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_device.h")
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
@@ -95,6 +96,13 @@ _LOOKUP_SIGS = {
     "ms_lookup_multiplicities": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ui, ui, ui, vp, sz, vp, vp]),
 }
 
+# include/ministark_permutation.h: target columns of the sorted-copy permutations an AIR declares (air.Permutation), filled
+# on the device
+_PERMUTATION_SIGS = {
+    "ms_permutation_workspace_bytes": (ci, [ui, ui, C.POINTER(sz)]),
+    "ms_permutation_fill": (ci, [vp, vp, ui, vp, ui, vp, vp, ui, ui, ui, vp, vp, sz]),
+}
+
 # include/ministark_bf.h: the execution trace of examples/brainfuck (VM on the host, tables on the device)
 _BF_SIGS = {
     "ms_bf_run": (ci, [vp, sz, vp, sz, u64, vp, vp, vp]),
@@ -154,6 +162,7 @@ def load():
         bind(lib, _CHECK_SIGS)
         bind(lib, _EXTENSION_SIGS)
         bind(lib, _LOOKUP_SIGS)
+        bind(lib, _PERMUTATION_SIGS)
         bind(lib, _BF_SIGS)
         bind(lib, _DEVICE_SIGS)
         bind(lib, _HOST_NODES_SIGS)

@@ -11,7 +11,8 @@ composition constraint only, CompositionCoeff(i) — the verifier randomness tha
 constants once the channel has produced it (src/air.rs:96-101).
 
 Extension columns may be declared the same way (AirConfig.extension_columns, RunningColumn): the prover then builds them
-on the device from the base trace instead of calling a host builder.
+on the device from the base trace instead of calling a host builder.  So may LogUp lookups (AirConfig.lookups, Lookup) and
+sorted-copy permutation arguments (AirConfig.permutations, Permutation), whose constraints the package generates.
 
 This module is pure bookkeeping (a few hundred DAG nodes): no field data is touched here.
 """
@@ -208,6 +209,43 @@ class Lookup:
     selectors: tuple = None
 
 
+MAX_PERMUTATION_WIDTH = 4                        # csrc/permutation.cu: at most this many words per tuple
+
+
+@dataclass(frozen=True)
+class Permutation:
+    """One sorted-copy permutation argument (AirConfig.permutations): the target columns hold the source tuples of every
+    row, sorted.  It is how a read/write memory is proven: the accesses in execution order are the source, the same
+    accesses sorted by (address, clock) the target, and the AIR's own constraints check the sorted table row by row.
+
+    source: W Exprs (or Fp values), 1 <= W <= 4.  They read Constant (Fp), X, Periodic and Trace(c, offset) of a base
+    column c at any offset (the row index wraps mod n); never a challenge, a hint, an extension column, a permutation's
+    target column or a lookup's multiplicity column, since the targets are filled before the base trace is committed.
+
+    target: W distinct base columns the prover writes: row j of target[k] holds word k of the j-th source tuple in
+    ascending lexicographic order of the canonical integers, word 0 first.  Equal tuples keep their row order (the sort
+    is stable), so an AIR that wants "by address, then clock" orders its tuple that way.  The targets are filled before
+    the lookups' multiplicities, so a lookup may read them.
+    running_product: an extension column the package declares and constrains.  AirConfig.extension_columns returns
+    None at its position.
+
+    Challenges: after the AIR's own and the lookups', permutation p (in declaration order) takes the next index as
+    alpha_p, and one more as beta_p only when W > 1.  Tuples are compressed as c(t) = t_0 + beta t_1 + beta^2 t_2 + ....
+    The running product is z_0 = 1, z_(i+1) = z_i (alpha - c(source_i)) / (alpha - c(target_i)), and three constraints are
+    appended after the lookups', per permutation: z_0 = 1; on every row but the last, the step with its denominator
+    cleared, z_(i+1) (alpha - c(target_i)) - z_i (alpha - c(source_i)); at the last row,
+    z_(n-1) (alpha - c(source_(n-1))) - (alpha - c(target_(n-1))).
+
+    Soundness: the fill is untrusted prover work, and the generated constraints prove only that the target rows are a
+    permutation of the source rows.  That the target is SORTED is not proven by the package: an AIR that relies on the
+    order must constrain it itself, for example with a range-check Lookup on the differences of its keys.  The
+    argument's error is at most about W n / |Fq| (Schwartz-Zippel in alpha and beta): with FQ_IS_FP = True and
+    n = 2^24 rows, about 2^-38."""
+    source: tuple
+    target: tuple
+    running_product: int
+
+
 class AirConfig:
     """Subclass and override, as with the reference's trait (src/air.rs:26-48).  Field values handed to and
     returned by the hooks are canonical integers (Fp) or 3-tuples of canonical integers (Fq3)."""
@@ -232,14 +270,20 @@ class AirConfig:
         """None (the trace builds its own extension columns), or one RunningColumn per extension column, in column
         order: the prover then builds them on the device from the base trace whenever the trace brings no builder of its
         own.  A declaration adds no constraint: the AIR's constraints must still enforce every declared column.  With
-        lookups: None at every lookup's running-sum position (the package declares those columns), or None as a whole
-        when every extension column is a lookup's running sum."""
+        lookups or permutations: None at every lookup's running-sum and every permutation's running-product position (the
+        package declares those columns), or None as a whole when every extension column is one of them."""
         return None
 
     @staticmethod
     def lookups(trace_len):
         """the AIR's LogUp lookups (Lookup), in declaration order.  The package generates their constraints and
         running-sum columns, and the prover fills their multiplicity columns on the device."""
+        return []
+
+    @staticmethod
+    def permutations(trace_len):
+        """the AIR's sorted-copy permutation arguments (Permutation), in declaration order.  The package generates their
+        constraints and running-product columns, and the prover fills their target columns on the device."""
         return []
 
 
@@ -253,7 +297,9 @@ class Air:
         self.constraints = list(config.constraints(trace_len))
         hook = getattr(config, "lookups", None)
         self.lookups = self._lookups(list(hook(trace_len)) if hook is not None else [])
-        self.constraints += self._lookup_constraints()
+        hook = getattr(config, "permutations", None)
+        self.permutations = self._permutations(list(hook(trace_len)) if hook is not None else [])
+        self.constraints += self._lookup_constraints() + self._permutation_constraints()
         # AirConfig::composition_constraint (src/air.rs:50-82)
         ce_blowup = max(blowup_factor(c, trace_len) for c in self.constraints)
         composition_degree = trace_len * ce_blowup - 1
@@ -271,7 +317,7 @@ class Air:
         self.ce_blowup_factor = blowup_factor(total, trace_len)
         assert self.ce_blowup_factor <= options.lde_blowup_factor
         hook = getattr(config, "extension_columns", None)
-        self.extension_declaration = self._declaration(self._merge_lookup_sums(hook(trace_len) if hook is not None else None))
+        self.extension_declaration = self._declaration(self._merge_generated(hook(trace_len) if hook is not None else None))
 
     def _lookups(self, decl):
         """AirConfig.lookups checked against the AIR: Lookups with Expr fields, or ValueError.  Also assigns each lookup its
@@ -311,6 +357,7 @@ class Air:
                               None if sel is None else tuple(_as_expr(e) for e in sel)))
             self.lookup_challenges.append((chal, chal + 1 if W > 1 else None))
             chal += 2 if W > 1 else 1
+        self._next_challenge = chal
         for l, lk in enumerate(out):
             named = [(f"table[{k}]", e) for k, e in enumerate(lk.table)]
             named += [(f"values[{q}][{k}]", e) for q, v in enumerate(lk.values) for k, e in enumerate(v)]
@@ -330,20 +377,88 @@ class Air:
                                          f"(0..{nbase - 1})")
         return out
 
-    def _compressed(self, l, tup):
-        """t_0 + beta t_1 + beta^2 t_2 + ... with lookup l's beta"""
+    def _permutations(self, decl):
+        """AirConfig.permutations checked against the AIR and its lookups: Permutations with Expr sources, or ValueError.
+        Also assigns each permutation its challenges (self.permutation_challenges: (alpha index, beta index or None)),
+        after the lookups'"""
+        cfg = self.config
+        nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
+        mults = {lk.multiplicity: l for l, lk in enumerate(self.lookups)}
+        sums = {lk.running_sum: l for l, lk in enumerate(self.lookups)}
+        chal = self._next_challenge
+        out, self.permutation_challenges = [], []
+        targets, products = {}, {}
+        for p, pm in enumerate(decl):
+            if not isinstance(pm, Permutation):
+                raise ValueError(f"permutation {p}: expected a Permutation, got {type(pm).__name__}")
+            source, target = tuple(pm.source), tuple(int(t) for t in pm.target)
+            W = len(source)
+            if not 1 <= W <= MAX_PERMUTATION_WIDTH:
+                raise ValueError(f"permutation {p}: source tuples of width {W}; 1 to {MAX_PERMUTATION_WIDTH} are supported")
+            if len(target) != W:
+                raise ValueError(f"permutation {p}: {len(target)} target columns for source tuples of width {W}")
+            for t in target:
+                if not 0 <= t < nbase:
+                    raise ValueError(f"permutation {p}: target column {t} is not a base column (0..{nbase - 1})")
+                if t in targets:
+                    who = "repeated" if targets[t] == p else f"also permutation {targets[t]}'s"
+                    raise ValueError(f"permutation {p}: target column {t} is {who}")
+                if t in mults:
+                    raise ValueError(f"permutation {p}: target column {t} is the multiplicity column of lookup {mults[t]}")
+                targets[t] = p
+            z = pm.running_product
+            if not nbase <= z < nbase + next_:
+                raise ValueError(f"permutation {p}: running-product column {z} is not an extension column "
+                                 f"({nbase}..{nbase + next_ - 1})")
+            if z in sums:
+                raise ValueError(f"permutation {p}: running-product column {z} is lookup {sums[z]}'s running sum")
+            if z in products:
+                raise ValueError(f"permutation {p}: running-product column {z} is also permutation {products[z]}'s")
+            products[z] = p
+            out.append(Permutation(tuple(_as_expr(e) for e in source), target, z))
+            self.permutation_challenges.append((chal, chal + 1 if W > 1 else None))
+            chal += 2 if W > 1 else 1
+        for p, pm in enumerate(out):
+            for k, e in enumerate(pm.source):
+                for kind, what in (("chal", "a challenge"), ("hint", "a hint"), ("ccoef", "a composition coefficient")):
+                    if _leaves(e, kind):
+                        raise ValueError(f"permutation {p}: source[{k}] reads {what}")
+                if any(ext for _, ext in _leaves(e, "const")):
+                    raise ValueError(f"permutation {p}: source[{k}] reads an extension-field constant")
+                for col, off in sorted(_leaves(e, "trace")):
+                    if col in targets:
+                        raise ValueError(f"permutation {p}: source[{k}] reads Trace({col}, {off}), a target column of "
+                                         f"permutation {targets[col]}")
+                    if col in mults:
+                        raise ValueError(f"permutation {p}: source[{k}] reads Trace({col}, {off}), the multiplicity column "
+                                         f"of lookup {mults[col]}")
+                    if not 0 <= col < nbase:
+                        raise ValueError(f"permutation {p}: source[{k}] reads Trace({col}, {off}), which is not a base "
+                                         f"column (0..{nbase - 1})")
+        return out
+
+    @staticmethod
+    def _compressed(beta, tup):
+        """t_0 + beta t_1 + beta^2 t_2 + ... with beta = Challenge(beta)"""
         acc = tup[0]
-        b = self.lookup_challenges[l][1]
         bpow = None
         for t in tup[1:]:
-            bpow = E.Challenge(b) if bpow is None else bpow * E.Challenge(b)
+            bpow = E.Challenge(beta) if bpow is None else bpow * E.Challenge(beta)
             acc = acc + bpow * t
         return acc
 
     def _lookup_denominators(self, l):
         lk = self.lookups[l]
-        alpha = E.Challenge(self.lookup_challenges[l][0])
-        return [alpha - self._compressed(l, lk.table)] + [alpha - self._compressed(l, v) for v in lk.values]
+        a, b = self.lookup_challenges[l]
+        alpha = E.Challenge(a)
+        return [alpha - self._compressed(b, lk.table)] + [alpha - self._compressed(b, v) for v in lk.values]
+
+    def _permutation_denominators(self, p):
+        """(alpha - c(source), alpha - c(target)) of permutation p"""
+        pm = self.permutations[p]
+        a, b = self.permutation_challenges[p]
+        alpha = E.Challenge(a)
+        return alpha - self._compressed(b, pm.source), alpha - self._compressed(b, [E.Trace(t, 0) for t in pm.target])
 
     def _lookup_constraints(self):
         """the three constraints of every lookup (Lookup), appended after the AIR's own.  With Q = 1, W = 1 and no selectors
@@ -375,34 +490,54 @@ class Air:
             out += [s / (x - first), (step - num) * but_last, (total + num) / (x - last)]
         return out
 
-    def _merge_lookup_sums(self, decl):
-        """the user's extension_columns with every lookup's running sum put in its place (RunningColumn(init=0,
-        add=m / d_0 - sum_q sigma_q / d_q)), or ValueError"""
-        if not self.lookups:
+    def _permutation_constraints(self):
+        """the three constraints of every permutation (Permutation), appended after the lookups'.  They are, node for node,
+        the ones examples/memory.py's MemoryAirConfig writes by hand."""
+        n = self.trace_len
+        g = domain_generator(self.log_n)
+        x, one = E.X(), E.Constant(1)
+        first, last = E.Constant(1), E.Constant(pow(g, n - 1, P))
+        but_last = (x - last) / (x ** n - one)
+        out = []
+        for p, pm in enumerate(self.permutations):
+            ds, dt = self._permutation_denominators(p)
+            z, z1 = E.Trace(pm.running_product, 0), E.Trace(pm.running_product, 1)
+            out += [(z - one) / (x - first), (z1 * dt - z * ds) * but_last, (z * ds - dt) / (x - last)]
+        return out
+
+    def _merge_generated(self, decl):
+        """the user's extension_columns with every lookup's running sum (RunningColumn(init=0, add=m / d_0 -
+        sum_q sigma_q / d_q)) and every permutation's running product (RunningColumn(init=1, mul=(alpha - c(source)) /
+        (alpha - c(target)))) put in its place, or ValueError"""
+        if not self.lookups and not self.permutations:
             return decl
         cfg = self.config
         nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
-        pos = {lk.running_sum - nbase: l for l, lk in enumerate(self.lookups)}
+        pos = {lk.running_sum - nbase: (f"lookup {l}'s running sum", l) for l, lk in enumerate(self.lookups)}
+        ppos = {pm.running_product - nbase: (f"permutation {p}'s running product", p) for p, pm in enumerate(self.permutations)}
         if decl is None:
-            if len(pos) != next_:
-                raise ValueError(f"extension_columns returned None, but only {len(pos)} of the {next_} extension columns "
-                                 f"are lookup running sums")
+            if len(pos) + len(ppos) != next_:
+                raise ValueError(f"extension_columns returned None, but only {len(pos) + len(ppos)} of the {next_} extension "
+                                 f"columns are lookup running sums or permutation running products")
             decl = [None] * next_
         decl = list(decl)
         if len(decl) != next_:
             raise ValueError(f"extension_columns declares {len(decl)} columns but NUM_EXTENSION_COLUMNS is {next_}")
         for k, col in enumerate(decl):
-            if k in pos and col is not None:
-                raise ValueError(f"extension column {nbase + k}: lookup {pos[k]}'s running sum is declared by the package; "
+            if (k in pos or k in ppos) and col is not None:
+                raise ValueError(f"extension column {nbase + k}: {(pos.get(k) or ppos[k])[0]} is declared by the package; "
                                  f"extension_columns must return None there")
-            if k not in pos and not isinstance(col, RunningColumn):
+            if k not in pos and k not in ppos and not isinstance(col, RunningColumn):
                 raise ValueError(f"extension column {nbase + k}: expected a RunningColumn, got {type(col).__name__}")
-        for k, l in pos.items():
+        for k, (_, l) in pos.items():
             lk, d = self.lookups[l], self._lookup_denominators(l)
             add = E.Trace(lk.multiplicity, 0) / d[0]
             for q, dq in enumerate(d[1:]):
                 add = add - (E.Constant(1) if lk.selectors is None else lk.selectors[q]) / dq
             decl[k] = RunningColumn(init=0, add=add)
+        for k, (_, p) in ppos.items():
+            ds, dt = self._permutation_denominators(p)
+            decl[k] = RunningColumn(init=1, mul=ds / dt)
         return decl
 
     def _declaration(self, decl):
@@ -492,6 +627,15 @@ class Air:
             self._lookup_programs = [E.compile_lookup_program(lk.table, lk.values, lk.selectors, nbase, self.log_n)
                                      for lk in self.lookups]
         return self._lookup_programs
+
+    def permutation_programs(self):
+        """one evaluator program per permutation, storing its source words, for its target fill (csrc/permutation.cu;
+        expr.compile_lookup_program with no value tuples)"""
+        if getattr(self, "_permutation_programs", None) is None:
+            nbase = self.config.NUM_BASE_COLUMNS
+            self._permutation_programs = [E.compile_lookup_program(pm.source, (), None, nbase, self.log_n)
+                                          for pm in self.permutations]
+        return self._permutation_programs
 
     # the three walks below depend on the constraints only: done once per Air (the provers copy a cached Air per proof,
     # and each walk of the brainfuck AIR costs ~0.5 ms of a 10 ms proof)

@@ -2,13 +2,11 @@
 // base trace with exact tuple matching.
 //
 // One call handles one lookup of W words per tuple (1..4) and Q value tuples (1..4) over n = 2^log_n rows:
-//   1. evaluate: one evaluator program (expr.py, compile_lookup_program) stores the W table words and, per value tuple,
-//      its selector and W words; eval.cuh's eval_point interprets it over the trace domain, one thread per row, and every
-//      output is written to the workspace as a canonical integer (never a lazy or Montgomery word), so equal field
-//      elements are equal words;
-//   2. order the table: W stable cub radix sorts of (word k gathered through the current permutation, row), from the last
-//      word to the first — an LSD lexicographic sort, so equal tuples end adjacent and in row order, the first row of a
-//      run being the lowest row holding that tuple; the sorted tuples are then gathered word by word;
+//   1. evaluate (tuples.cuh, tuple_evaluate): one evaluator program (expr.py, compile_lookup_program) stores the W table
+//      words and, per value tuple, its selector and W words, as canonical integers in the workspace's slot columns;
+//   2. order the table (tuples.cuh, tuple_sort): an LSD lexicographic sort of W stable radix passes, so equal tuples end
+//      adjacent and in row order, the first row of a run being the lowest row holding that tuple; the sorted tuples are
+//      then gathered word by word;
 //   3. match: one thread per (row, value tuple).  Selector 0: nothing.  A selector that is neither 0 nor 1 is counted as
 //      bad.  Otherwise a lexicographic lower-bound binary search in the sorted table; a hit adds 1 to the 64-bit counter of
 //      the run's first row (threads of a warp that hit the same row add once, together), a miss is counted for the tuple;
@@ -16,23 +14,18 @@
 // Rows and offsets into the workspace are 64-bit throughout.  Traffic per row: the cells the program reads, the S =
 // W + Q (W + 1) slot words written once and read once or twice, 16 W bytes of keys and 8 W of permutation per sort pass
 // (plus cub's 8-bit digit passes), and W sorted words per search step (log2 n steps, cached near the root).
-#include "eval.cuh"
+#include "tuples.cuh"
 #include "../../include/ministark_lookup.h"
-
-#include <cub/cub.cuh>
-#include <vector>
 
 namespace ms {
 
 constexpr unsigned kMaxLookupWidth = 4, kMaxLookupTuples = 4, kMaxLookupLog = 30;
-constexpr int kLookupThreads = 256;
+constexpr int kLookupThreads = kTupleThreads;
 
 // workspace layout (byte offsets, each region 256-byte aligned)
 struct LookupWork {
     size_t slots, sorted, keys, perm, status, total;
 };
-
-static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 static LookupWork lookup_layout(unsigned log_n, unsigned W, unsigned Q) {
     const size_t n = (size_t)1 << log_n, S = (size_t)W + (size_t)Q * (W + 1);
@@ -44,42 +37,6 @@ static LookupWork lookup_layout(unsigned log_n, unsigned W, unsigned Q) {
     w.status = w.perm + align256(2 * n * 4);
     w.total = w.status + align256((2 * kMaxLookupTuples + 2) * 8);
     return w;
-}
-
-struct LookupEvalParams {
-    // the fields eval_point reads
-    const uint4 *prog;
-    u32 nprog;
-    const u64 *consts;
-    const u64 *const *col_ptr;
-    u32 fq_words;               // 1: every expression is over Fp
-    u32 log_m;
-    u32 trace_bitrev;           // 0: natural order
-    const u64 *tw_lo, *tw_hi;
-    u32 hi_len;
-    u64 offset;                 // ONE: X is g_n^i
-    u64 *slots;                 // slot s of row i at slots[s * n + i], canonical
-};
-
-__global__ void __launch_bounds__(kLookupThreads) lookup_eval_kernel(const LookupEvalParams p) {
-    const u64 n = 1ull << p.log_m;
-    const u64 i = (u64)blockIdx.x * kLookupThreads + threadIdx.x;
-    if (i >= n) return;
-    u64 r[kMaxRegs][3];
-    eval_point(p, n, i, r, [&](u32 s, const u64 *v, bool) { p.slots[(u64)s * n + i] = gl::canon(gl::from_mont(v[0])); });
-}
-
-// key[j] = word[perm[j]] (perm == nullptr: key[j] = word[j] and perm_out[j] = j)
-__global__ void __launch_bounds__(kLookupThreads) lookup_gather_kernel(const u64 *word, const u32 *perm, u64 *key, u32 *perm_out,
-                                                                       u64 n) {
-    const u64 j = (u64)blockIdx.x * kLookupThreads + threadIdx.x;
-    if (j >= n) return;
-    if (perm) {
-        key[j] = word[perm[j]];
-    } else {
-        key[j] = word[j];
-        perm_out[j] = (u32)j;
-    }
 }
 
 template <int W>
@@ -181,38 +138,20 @@ extern "C" int ms_lookup_multiplicities(ms_ctx *c, const uint32_t *program, unsi
     if (workspace_bytes < w.total)
         return fail(c, MS_ERR_INVALID, "ms_lookup_multiplicities: workspace of %zu bytes, %zu needed", workspace_bytes, w.total);
     cudaSetDevice(c->device);
-    std::vector<const u64 *> cols;
-    std::vector<int> isq;
-    for (unsigned k = 0; k < ncols; k++) {
-        if (!col_ptrs[k] || !is_device_ptr(col_ptrs[k])) return fail(c, MS_ERR_INVALID, "ms_lookup_multiplicities: column %u is not a device pointer", k);
-        if (col_is_fq[k]) return fail(c, MS_ERR_INVALID, "ms_lookup_multiplicities: column %u is not a base-field column", k);
-        cols.push_back((const u64 *)col_ptrs[k]);
-        isq.push_back(0);
-    }
     if (!is_device_ptr(workspace) || !is_device_ptr(out))
         return fail(c, MS_ERR_INVALID, "ms_lookup_multiplicities: workspace and out must be device pointers");
-    const unsigned nslots = width + ntuples * (width + 1);
-    int rc = validate_program(c, "ms_lookup_multiplicities", program, nprog, nconsts, isq, log_n, 0, nslots);
-    if (rc) return rc;
-    for (unsigned k = 0; k < nprog; k++)
-        if ((program[4 * k] & 0xff) == OP_STORE && ((program[4 * k] >> 8) & 1))
-            return fail(c, MS_ERR_INVALID, "ms_lookup_multiplicities: instruction %u stores an extension-field value", k);
-    void *meta;
-    const size_t prog_bytes = (size_t)nprog * 16, const_bytes = (size_t)nconsts * 24, ptr_bytes = (size_t)ncols * 8;
-    if ((rc = scratch_get(c, 3, prog_bytes + const_bytes + ptr_bytes + 64, &meta))) return rc;
-    char *m = (char *)meta;
-    // pageable host sources: each copy returns once its source is staged, so the caller's buffers are free afterwards
-    MS_CUDA(c, cudaMemcpyAsync(m, program, prog_bytes, cudaMemcpyDefault, c->stream));
-    MS_CUDA(c, cudaMemcpyAsync(m + prog_bytes, consts, const_bytes, cudaMemcpyDefault, c->stream));
-    if (ptr_bytes) MS_CUDA(c, cudaMemcpyAsync(m + prog_bytes + const_bytes, cols.data(), ptr_bytes, cudaMemcpyHostToDevice, c->stream));
-
     const u64 n = 1ull << log_n;
-    const unsigned nblk = (unsigned)((n + kLookupThreads - 1) / kLookupThreads);
+    const unsigned nblk = tuple_blocks(n);
     char *wb = (char *)workspace;
     u64 *slots = (u64 *)(wb + w.slots), *sorted = (u64 *)(wb + w.sorted), *st = (u64 *)(wb + w.status);
     u64 *keys0 = (u64 *)(wb + w.keys), *keys1 = keys0 + n;
     u32 *perm0 = (u32 *)(wb + w.perm), *perm1 = perm0 + n;
     u64 *counts = (u64 *)out;
+
+    // 1. evaluate
+    int rc = tuple_evaluate(c, "ms_lookup_multiplicities", program, nprog, consts, nconsts, col_ptrs, col_is_fq, ncols, log_n,
+                            width + ntuples * (width + 1), slots);
+    if (rc) return rc;
     std::vector<u64> init(2 * ntuples + 2);
     for (unsigned k = 0; k < ntuples + 1; k++) {
         init[2 * k] = 0;
@@ -221,50 +160,21 @@ extern "C" int ms_lookup_multiplicities(ms_ctx *c, const uint32_t *program, unsi
     MS_CUDA(c, cudaMemcpyAsync(st, init.data(), init.size() * 8, cudaMemcpyHostToDevice, c->stream));
     MS_CUDA(c, cudaMemsetAsync(counts, 0, n * 8, c->stream));
 
-    // 1. evaluate
-    LookupEvalParams p;
-    if ((rc = ntt_plan_tables(c, log_n, &p.tw_lo, &p.tw_hi, &p.hi_len))) return rc;
-    p.prog = (const uint4 *)m;
-    p.nprog = nprog;
-    p.consts = (const u64 *)(m + prog_bytes);
-    p.col_ptr = (const u64 *const *)(m + prog_bytes + const_bytes);
-    p.fq_words = 1;
-    p.log_m = log_n;
-    p.trace_bitrev = 0;
-    p.offset = gl::ONE;
-    p.slots = slots;
-    lookup_eval_kernel<<<nblk, kLookupThreads, 0, c->stream>>>(p);
-    c->launches++;
-    MS_CHECK_LAUNCH(c);
-
-    // 2. LSD lexicographic sort of the table: stable passes from the last word to the first
-    cub::DoubleBuffer<u64> keys(keys0, keys1);
-    cub::DoubleBuffer<u32> perm(perm0, perm1);
-    size_t tb = 0;
-    MS_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, perm, (int)n, 0, 64, c->stream));
-    void *temp;
-    if ((rc = scratch_get(c, 2, tb, &temp))) return rc;
-    for (int k = (int)width - 1; k >= 0; k--) {
-        const bool first = k == (int)width - 1;
-        lookup_gather_kernel<<<nblk, kLookupThreads, 0, c->stream>>>(slots + (u64)k * n, first ? nullptr : perm.Current(),
-                                                                    keys.Current(), perm.Current(), n);
-        c->launches++;
-        MS_CHECK_LAUNCH(c);
-        MS_CUDA(c, cub::DeviceRadixSort::SortPairs(temp, tb, keys, perm, (int)n, 0, 64, c->stream));
-    }
+    // 2. order the table, then gather its tuples word by word
+    const u32 *order;
+    if ((rc = tuple_sort(c, slots, width, n, keys0, keys1, perm0, perm1, &order))) return rc;
     for (unsigned k = 0; k < width; k++) {
-        lookup_gather_kernel<<<nblk, kLookupThreads, 0, c->stream>>>(slots + (u64)k * n, perm.Current(), sorted + (u64)k * n,
-                                                                    nullptr, n);
+        tuple_gather_kernel<<<nblk, kTupleThreads, 0, c->stream>>>(slots + (u64)k * n, order, sorted + (u64)k * n, nullptr, n);
         c->launches++;
     }
     MS_CHECK_LAUNCH(c);
 
     // 3. match
     switch (width) {
-        case 1: rc = lookup_match<1>(c, slots, sorted, perm.Current(), n, ntuples, counts, st); break;
-        case 2: rc = lookup_match<2>(c, slots, sorted, perm.Current(), n, ntuples, counts, st); break;
-        case 3: rc = lookup_match<3>(c, slots, sorted, perm.Current(), n, ntuples, counts, st); break;
-        default: rc = lookup_match<4>(c, slots, sorted, perm.Current(), n, ntuples, counts, st); break;
+        case 1: rc = lookup_match<1>(c, slots, sorted, order, n, ntuples, counts, st); break;
+        case 2: rc = lookup_match<2>(c, slots, sorted, order, n, ntuples, counts, st); break;
+        case 3: rc = lookup_match<3>(c, slots, sorted, order, n, ntuples, counts, st); break;
+        default: rc = lookup_match<4>(c, slots, sorted, order, n, ntuples, counts, st); break;
     }
     if (rc) return rc;
 

@@ -417,7 +417,8 @@ def compile_lookup_program(table, values, selectors, num_base_cols, log_n):
     value tuple q's selector (Constant 1 without selectors) to slot W + q (W + 1) and its word k to the slot k + 1 after
     that.  Every expression is over the base field: Trace(col, off) reads column[(i + off) mod 2^log_n] of the
     natural-order trace, X is g_n^i, periodic tables come from periodic_tables(ctx, program, log_n, 1,
-    offset_canonical=1)."""
+    offset_canonical=1).  With no value tuples it stores a permutation's W source words (air.Permutation,
+    csrc/permutation.cu)."""
     W = len(table)
     roots = [Expr._lift(t) for t in table]
     for q, v in enumerate(values):

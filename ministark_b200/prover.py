@@ -193,13 +193,34 @@ def fill_lookup_multiplicities(ctx, air, base):
         raise LookupViolation(misses)
 
 
+def fill_permutation_targets(ctx, air, base):
+    """the target columns of every permutation `air` declares (AirConfig.permutations), written into `base`
+    ((NUM_BASE_COLUMNS, n) natural-order device tensor, the prover's own copy) by ms_permutation_fill, one call per
+    permutation in declaration order with the cached programs"""
+    nbase, log_n = air.config.NUM_BASE_COLUMNS, air.log_n
+    for pm, prog in zip(air.permutations, air.permutation_programs()):
+        W = len(pm.source)
+        work = torch.empty(ctx.permutation_workspace_bytes(log_n, W), dtype=torch.uint8, device=base.device)
+        tables = E.periodic_tables(ctx, prog, log_n, 1, offset_canonical=1)
+        try:
+            ctx.permutation_fill(prog, [base[t] for t in pm.target], log_n,
+                                 [base[c] for c in range(nbase)] + [p for p, _ in tables], W, work)
+        finally:
+            if tables:
+                ctx.sync()
+            for p, _ in tables:
+                ctx.free(p)
+        del work                                # freed in stream order: the fill runs on the prover's stream
+
+
 def check_lookup_trace(air, trace):
-    """a trace that builds its own extension columns cannot know the multiplicities the prover fills: refused for an AIR
-    with lookups, before anything is computed"""
-    if air.lookups and (hasattr(trace, "build_extension_columns_device") or getattr(trace, "_ext", None) is not None
-                        or type(trace).build_extension_columns is not Trace.build_extension_columns):
-        raise ProvingError("the AIR declares lookups, whose running sums the package builds from the multiplicities it fills; "
-                           "the trace must not bring its own extension columns")
+    """a trace that builds its own extension columns cannot know the columns the prover fills (lookup multiplicities,
+    permutation targets): refused for an AIR with lookups or permutations, before anything is computed"""
+    if (air.lookups or air.permutations) and (
+            hasattr(trace, "build_extension_columns_device") or getattr(trace, "_ext", None) is not None
+            or type(trace).build_extension_columns is not Trace.build_extension_columns):
+        raise ProvingError("the AIR declares lookups or permutations, whose running columns the package builds from the "
+                           "columns it fills; the trace must not bring its own extension columns")
 
 
 class _Tree:
@@ -470,7 +491,7 @@ class GpuProver:
             nonlocal t0
             ctx.sync()
             t = time.perf_counter()
-            if since is not None:           # lookup_multiplicities: timed on its own, outside the phase it runs in
+            if since is not None:           # permutation_fill, lookup_multiplicities: timed on their own, outside the phase
                 timings[name] = t - since
                 t0 += t - since
                 return
@@ -494,6 +515,7 @@ class GpuProver:
             self._airs[key].deep_program()
             self._airs[key].extension_program()
             self._airs[key].lookup_programs()
+            self._airs[key].permutation_programs()
             self._airs[key].num_challenges(), self._airs[key].num_composition_constraint_coeffs(), self._airs[key].trace_arguments()
         air = copy.copy(self._airs[key])
         air.public_inputs = stark.get_public_inputs()
@@ -523,8 +545,8 @@ class GpuProver:
         # while the previous chunk is interpolated and extended (columns are independent until the row hash); a
         # pinned trace — the analogue of the reference's GpuAllocator-backed columns — makes the copies asynchronous.
         host_base = self._base_columns(r)
-        if air.lookups:
-            # the multiplicities are filled before the commitment, so the upload cannot overlap the transforms here
+        if air.lookups or air.permutations:
+            # the filled columns are written before the commitment, so the upload cannot overlap the transforms here
             base = self._lookup_base(r, host_base)
             base_polys, base_lde, base_tree, base_root = self._commit_columns(base, FP, log_n, log_b, nbase, True)
         elif isinstance(host_base, torch.Tensor) and host_base.is_cuda:
@@ -680,7 +702,7 @@ class GpuProver:
 
         # ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
         host_base = self._base_columns(r)
-        base = self._lookup_base(r, host_base) if air.lookups else self._to_device(host_base)
+        base = self._lookup_base(r, host_base) if air.lookups or air.permutations else self._to_device(host_base)
         del host_base                           # held no longer than `base`: see release_base_columns below
         base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
         ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
@@ -772,13 +794,20 @@ class GpuProver:
 
     # ---- phases every driver shares (ShardedProver included)
     def _lookup_base(self, r, host_base):
-        """the prover's own device copy of the base columns (the caller's trace, host or device, is never written) with
-        every lookup's multiplicity column filled; timed as timings["lookup_multiplicities"]"""
+        """the prover's own device copy of the base columns (the caller's trace, host or device, is never written) with the
+        columns the AIR leaves to the package filled: every permutation's targets first, in declaration order, then every
+        lookup's multiplicity column (a lookup may read a target).  Timed as timings["permutation_fill"] and
+        timings["lookup_multiplicities"]"""
         base = self._own_copy(host_base)
         r.ctx.sync()
-        t = time.perf_counter()
-        fill_lookup_multiplicities(r.ctx, r.air, base)
-        r.lap("lookup_multiplicities", since=t)
+        if r.air.permutations:
+            t = time.perf_counter()
+            fill_permutation_targets(r.ctx, r.air, base)
+            r.lap("permutation_fill", since=t)
+        if r.air.lookups:
+            t = time.perf_counter()
+            fill_lookup_multiplicities(r.ctx, r.air, base)
+            r.lap("lookup_multiplicities", since=t)
         return base
 
     def _keep_for_check(self, r, base, ext):

@@ -25,9 +25,9 @@ once and finished on every rank.  torch / torch.distributed are plumbing: buffer
 
 ShardedProver is a GpuProver: only what depends on where the LDE rows live is written here (the column-split
 interpolation, the slab LDE and commitment, the block-wise constraint evaluation and DEEP, the sharded FRI layers and
-the query fetch plan).  The set-up, the phase clock, the base-column read, the lookup fill, the extension and
-composition columns, the OOD/DEEP binding, the gathered FRI layers, the remainder and proof of work, and the proof
-assembly are GpuProver's methods, shared with its resident and streamed drivers.
+the query fetch plan).  The set-up, the phase clock, the base-column read, the permutation and lookup fills, the
+extension and composition columns, the OOD/DEEP binding, the gathered FRI layers, the remainder and proof of work, and
+the proof assembly are GpuProver's methods, shared with its resident and streamed drivers.
 """
 import hashlib
 
@@ -303,8 +303,8 @@ class ShardedProver(GpuProver):
         host_base = self._base_columns(r)
         needs_full_base = next_ > 0          # extension columns are built from the whole base trace (on every rank)
         if needs_full_base or nbase < G or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
-            # with lookups every rank fills its own copy (a lookup always has an extension column)
-            base = self._lookup_base(r, host_base) if air.lookups else self._to_device(host_base)
+            # with lookups or permutations every rank fills its own copy (each has an extension column)
+            base = self._lookup_base(r, host_base) if air.lookups or air.permutations else self._to_device(host_base)
             base_polys = self._interpolate(base, FP, nbase, log_n)
         else:
             base = None
