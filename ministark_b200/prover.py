@@ -320,10 +320,38 @@ def _gib(b):
 
 
 class _Run:
-    """per-proof state shared by the phases of every driver (resident, streamed, sharded)"""
+    """per-proof state shared by the phases of every residency (resident, streamed, sharded)"""
 
     def __init__(self, **kw):
         self.__dict__.update(kw)
+
+
+class _Matrix:
+    """a committed matrix: its coefficients, its LDE rows where the residency keeps them (the whole bit-reversed LDE
+    when resident, one coset-block buffer when streamed, this rank's slab when sharded), its Merkle tree and root"""
+
+    def __init__(self, polys, rows, field, ncols, tree=None, root=None):
+        self.polys, self.rows, self.field, self.ncols, self.tree, self.root = polys, rows, field, ncols, tree, root
+
+
+class _Layout:
+    """where one proof's LDE rows live: the steps of GpuProver._default_prove that depend on it"""
+
+    def __init__(self, prover, r):
+        self.p, self.r = prover, r
+
+    def fri(self, codeword):
+        """FRI layers (fri.rs:179-249), the remainder and the proof of work; returns the committed layers"""
+        r = self.r
+        log_ff = r.options.fri_folding_factor.bit_length() - 1
+        layers = []
+        cur, ln = codeword, r.log_N
+        for _ in range(r.options.fri_num_layers(r.N)):
+            layer, cur = self.p._fri_layer(r, cur, ln)
+            layers.append(layer)
+            ln -= log_ff
+        self.p._fri_tail(r, cur, ln)
+        return layers
 
 
 class GpuProver:
@@ -396,21 +424,6 @@ class GpuProver:
     def _empty(self, *shape):
         return torch.empty(shape, dtype=torch.int64, device=self.device)
 
-    def _commit_columns(self, polys_in, field, log_n, log_b, ncols, is_evals):
-        """interpolate (if is_evals) + bit-reversed LDE + Merkle commit of a column-major matrix.
-        Returns (polys, lde, tree, root)."""
-        ctx, n, N = self.ctx, 1 << log_n, 1 << (log_n + log_b)
-        if is_evals:
-            polys = self._empty(ncols, n * field)
-            ctx.ntt_batch_to(polys_in, polys, field, log_n, ncols, inverse=True)      # Matrix::interpolate over the trace domain
-        else:
-            polys = polys_in
-        lde = self._empty(ncols, N * field)
-        ctx.lde_batch(polys, lde, field, log_n, log_b, ncols, offset=GEN_MONT, bitrev=True)
-        leaves, nodes = self._empty(N, 4), self._empty(N, 4)
-        root = ctx.merkle_commit(lde, field, N, ncols, leaves=leaves, nodes=nodes)
-        return polys, lde, _Tree(leaves, nodes, N), root
-
     def _view(self, tree, positions):
         nodes, init, sib, height = self.ctx.merkle_prove(tree.leaves, tree.nodes, tree.n, positions)
         return MerkleView(nodes, init, sib, height)
@@ -465,15 +478,16 @@ class GpuProver:
         self.last_residency = residency
         r.lap("init_air")
         if residency == "resident":
-            return self._prove_resident(r)
+            return self._default_prove(r, _Resident(self, r))
+        host_heaps = None
         if residency == "streamed_host":
             # tree t's node heap: beta local heaps of n digests (base, extension if any, composition)
-            r.host_heaps = self._host_heaps(est["host"])[:est["host"]].reshape(-1, r.beta, r.n, 32)
+            host_heaps = self._host_heaps(est["host"])[:est["host"]].reshape(-1, r.beta, r.n, 32)
             r.lap("pin_host_memory")
-        return self._prove_streamed(r)
+        return self._default_prove(r, _Streamed(self, r, host_heaps))
 
     def _start(self, stark, options, witness, validate):
-        """the set-up every driver shares: the trace, the cached Air with its compiled programs, this proof's public
+        """the set-up every residency shares: the trace, the cached Air with its compiled programs, this proof's public
         inputs, the shapes, the channel and the phase clock (r.lap).  Returns the _Run with the phase "init_air" open; the
         trace's columns are not read yet."""
         ctx = self.ctx
@@ -526,9 +540,11 @@ class GpuProver:
         log_b = beta.bit_length() - 1
         nbase, next_ = cfg.NUM_BASE_COLUMNS, cfg.NUM_EXTENSION_COLUMNS
         channel = ProverChannel(air, stark.gen_public_coin(air), ctx)
+        ce_blowup = air.ce_blowup_factor
         return _Run(ctx=ctx, stark=stark, options=options, trace=trace, air=air, channel=channel, fq=fq, n=n, log_n=log_n,
-                    beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_, lap=lap,
-                    timings=timings, t_all=t_all, cached_air=self._airs[key], validate=validate, host_heaps=None)
+                    beta=beta, log_b=log_b, log_N=log_n + log_b, N=n * beta, nbase=nbase, next_=next_,
+                    ce_blowup=ce_blowup, log_ce=log_n + ce_blowup.bit_length() - 1, lap=lap, timings=timings,
+                    t_all=t_all, cached_air=self._airs[key], validate=validate)
 
     def _base_columns(self, r):
         """the trace's base columns, refused unless they are (NUM_BASE_COLUMNS, n)"""
@@ -537,262 +553,67 @@ class GpuProver:
             raise ProvingError(f"expected {r.nbase} base columns of {r.n} rows")
         return base
 
-    def _prove_resident(self, r):
-        ctx, air, channel, lap = r.ctx, r.air, r.channel, r.lap
-        fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
+    def _default_prove(self, r, rows):
+        """default_prove (src/prover.rs:40-174) after the set-up: every commitment, Fiat–Shamir draw and phase in the
+        reference's order, for every residency.  `rows` (_Resident, _Streamed, prover_mgpu._Sharded) does the steps that
+        depend on where the LDE rows live: the commitments, the evaluations over the LDE, FRI and the queried rows."""
+        air, channel, lap, fq = r.air, r.channel, r.lap, r.fq
 
-        # ---- base trace commitment (prover.rs:46-55).  A host trace is uploaded in column chunks on a second stream
-        # while the previous chunk is interpolated and extended (columns are independent until the row hash); a
-        # pinned trace — the analogue of the reference's GpuAllocator-backed columns — makes the copies asynchronous.
-        host_base = self._base_columns(r)
-        if air.lookups or air.permutations:
-            # the filled columns are written before the commitment, so the upload cannot overlap the transforms here
-            base = self._lookup_base(r, host_base)
-            base_polys, base_lde, base_tree, base_root = self._commit_columns(base, FP, log_n, log_b, nbase, True)
-        elif isinstance(host_base, torch.Tensor) and host_base.is_cuda:
-            base = host_base.to(self.device)
-            base_polys, base_lde, base_tree, base_root = self._commit_columns(base, FP, log_n, log_b, nbase, True)
-        else:
-            if not isinstance(host_base, torch.Tensor):
-                host_base = torch.from_numpy(np.ascontiguousarray(host_base, dtype=np.uint64).view(np.int64))
-            base, base_polys, base_lde = self._empty(nbase, n), self._empty(nbase, n), self._empty(nbase, N)
-            chunk = max(1, min(nbase, (64 << 20) // (8 * n) or 1))            # ~64 MiB per copy
-            self.copy_stream.wait_stream(self.stream)
-            events = []
-            with torch.cuda.stream(self.copy_stream):
-                for c0 in range(0, nbase, chunk):
-                    c1 = min(c0 + chunk, nbase)
-                    base[c0:c1].copy_(host_base[c0:c1], non_blocking=True)
-                    ev = torch.cuda.Event()
-                    ev.record(self.copy_stream)
-                    events.append((c0, c1, ev))
-            for c0, c1, ev in events:
-                self.stream.wait_event(ev)
-                ctx.ntt_batch_to(base[c0], base_polys[c0], FP, log_n, c1 - c0, inverse=True)
-                ctx.lde_batch(base_polys[c0], base_lde[c0], FP, log_n, log_b, c1 - c0, offset=GEN_MONT, bitrev=True)
-            leaves, nodes = self._empty(N, 4), self._empty(N, 4)
-            base_root = ctx.merkle_commit(base_lde, FP, N, nbase, leaves=leaves, nodes=nodes)
-            base_tree = _Tree(leaves, nodes, N)
-        del host_base                           # held no longer than `base`: see release_base_columns below
-        channel.commit_base_trace(base_root)
+        # ---- base trace commitment (prover.rs:46-55)
+        base, base_m = rows.commit_base()
+        channel.commit_base_trace(base_m.root)
         lap("base_trace_commitment")
         challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
         hints = air.gen_hints(challenges)
 
         # ---- extension trace commitment (prover.rs:56-72)
         ext = self._extension_columns(r, challenges, hints, base)
-        check = self._keep_for_check(r, base, ext)
+        # with validation: the natural-order base columns and the extension columns on the device (a host-built extension
+        # matrix uploaded once, for the check and the commitment), kept until the check has run
+        check = (base, None if ext is None else self._to_device(ext)) if r.validate else None
         del base
-        ext_polys = ext_lde = ext_tree = None
+        ext_m = None
         if ext is not None:
-            ext = check[1] if check else ext           # with validation: the one device copy serves both
-            ext_polys, ext_lde, ext_tree, ext_root = self._commit_columns(self._to_device(ext), fq, log_n, log_b, next_, True)
-            channel.commit_extension_trace(ext_root)
+            # large buffers are handed to the layout in a list it may empty: the streamed layout frees them as soon as it
+            # has their coefficients, the others when this list goes
+            ext = [check[1] if check else ext]          # with validation: the one device copy serves both
+            ext_m = rows.commit_evals(ext, fq, r.next_)
+            channel.commit_extension_trace(ext_m.root)
         del ext
         lap("extension_trace_commitment")
-        self._check(r, challenges, hints, check)
+        if check is not None:                   # Stark::validate_constraints at the reference's position (src/prover.rs:74-75)
+            air._check_program = r.cached_air.check_program()        # compiled once per AIR and trace length
+            r.stark.validate_constraints(air, challenges, hints, check[0], check[1], r.ctx)
+            lap("validate_constraints")
         del check
 
-        # ---- constraint evaluation over the ce domain (prover.rs:75-108).  The first M entries of a bit-reversed LDE
-        # column ARE the ce-coset evaluations in bit-reversed order, so they are read in place (trace_bitrev).
-        ce_blowup = air.ce_blowup_factor
-        log_ce = log_n + ce_blowup.bit_length() - 1
-        M = n * ce_blowup
+        # ---- constraint evaluation over the ce domain (prover.rs:75-108)
         composition_coeffs = [channel.public_coin.draw() for _ in range(air.num_composition_constraint_coeffs())]
-        prog = air.composition_program().bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
-        comp_evals = self._empty(M * fq)
-        ctx.eval_constraints(prog, comp_evals, log_ce, base_cols=base_lde, nbase=nbase, base_stride=N,
-                             ext_cols=ext_lde, next_=next_, ext_stride=N, fq_field=fq, offset=GEN_MONT, trace_bitrev=True)
+        comp_evals = [rows.constraint_evals(base_m, ext_m, dict(challenges=challenges, hints=hints, ccoefs=composition_coeffs))]
         lap("constraint_eval")
 
-        # ---- composition trace (prover.rs:110-125): coefficients over the ce coset, column i = coefficients = i mod ce_blowup
-        ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
-        comp_polys = self._composition_columns(r, comp_evals)
-        _, comp_lde, comp_tree, comp_root = self._commit_columns(comp_polys, fq, log_n, log_b, ce_blowup, False)
-        channel.commit_composition_trace(comp_root)
+        # ---- composition trace (prover.rs:110-125)
+        comp_m = rows.commit_coeffs(rows.composition_polys(comp_evals), fq, r.ce_blowup)
+        channel.commit_composition_trace(comp_m.root)
         lap("composition_trace_commitment")
 
         # ---- DEEP composition polynomial, evaluated straight over the LDE domain (composer.rs:89-188 in evaluation form)
-        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
-        ncols_all = nbase + next_ + ce_blowup
-        sz = N * 8
-        cols = [base_lde.data_ptr() + c * sz for c in range(nbase)]
-        cols += [ext_lde.data_ptr() + c * sz * fq for c in range(next_)]
-        cols += [comp_lde.data_ptr() + c * sz * fq for c in range(ce_blowup)]
-        deep_lde = self._empty(N * fq)
-        ctx.eval_constraints_ptrs(dprog, deep_lde, r.log_N, cols, [False] * nbase + [True] * (ncols_all - nbase), fq_field=fq,
-                                  offset=GEN_MONT, trace_bitrev=True, out_bitrev=True)
+        mats = (base_m, ext_m, comp_m)
+        dprog = self._bind_deep(r, base_m.polys, ext_m.polys if ext_m else None, comp_m.polys)
+        codeword = rows.deep_codeword(dprog, mats)
         lap("deep_composition")
 
-        layers = self._fri(r, deep_lde)
+        layers = rows.fri(codeword)             # FRI layers, the remainder and the proof of work (fri.rs:179-249)
 
         # ---- queries (fri.rs:151-177, trace.rs:115-157)
         positions = channel.get_fri_query_positions()
-        fri_proof = self._fri_queries(r, layers, positions)
-        queries = Queries(
-            _canon_rows(ctx.gather_rows(base_lde, FP, N, nbase, positions), 1),
-            _canon_rows(ctx.gather_rows(ext_lde, fq, N, next_, positions), fq) if next_ else [],
-            _canon_rows(ctx.gather_rows(comp_lde, fq, N, ce_blowup, positions), fq),
-            self._view(base_tree, positions),
-            self._view(ext_tree, positions) if next_ else None,
-            self._view(comp_tree, positions))
-        return self._finish(r, fri_proof, queries)
-
-    # ---- streamed residency: coefficients and tree nodes stay, coset blocks are recomputed
-    def _commit_blocks(self, polys, blk, field, ncols, log_n, log_b, offsets, host_heap=None):
-        """Merkle commitment of the bit-reversed LDE of `polys`, one coset block at a time: block q is transformed into
-        `blk` and hashed into its subtree of the node heap; the top log_b levels come from the block roots.
-        Returns (nodes, root).  With host_heap ((beta, n, 32) bytes of pinned host memory), block q's subtree is its local
-        heap host_heap[q] and nodes is (top heap of 2 beta digests on the host, host_heap): the split layout of
-        include/ministark_host_nodes.h."""
-        ctx, beta = self.ctx, 1 << log_b
-        if host_heap is None:
-            nodes, roots = self._empty(beta << log_n, 4), self._empty(beta, 4)
-        else:
-            nodes = self._empty(2 * beta, 4)
-            roots = nodes[beta:]
-        for q, h in offsets:
-            self._block(polys, blk, field, ncols, log_n, h)
-            if host_heap is None:
-                ctx.merkle_commit_block(blk, field, log_n, log_b, q, ncols, nodes, roots[q])
-            else:
-                ctx.merkle_commit_block_host(blk, field, log_n, ncols, host_heap[q], roots[q])
-        if beta > 1:
-            ctx.merkle_nodes(roots, nodes, beta)
-        nodes[0].zero_()                        # the unused default digest (named by a walk over a 2-leaf tree)
-        root = nodes[1].cpu().numpy().tobytes()
-        if host_heap is not None:
-            nodes = (nodes.cpu().numpy().view(np.uint8), host_heap)
-        return nodes, root
-
-    def _block(self, polys, blk, field, ncols, log_n, h):
-        """coset block with offset h of the bit-reversed LDE of every column of `polys`, into `blk`.  Its NTT plan is
-        dropped at once: every block has its own offset, and beta cached plans with their full tables (up to GiBs each
-        at 2^24 points) would take back the memory streaming saves"""
-        self.ctx.lde_batch(polys, blk, field, log_n, 0, ncols, offset=h, bitrev=True)
-        self.ctx.set_option("drop_plans", 1)
-
-    def _streamed_queries(self, polys, field, ncols, nodes, log_n, log_b, positions):
-        """the rows at `positions` and their MerkleView without the LDE: rows and leaf digests from the coefficients
-        (ms_lde_rows), path nodes gathered from the resident node heap"""
-        N = 1 << (log_n + log_b)
-        init, sib, path = merkle_walk(N, positions)
-        k = len(positions)
-        rows = self.ctx.lde_rows(polys, field, log_n, log_b, ncols, list(positions) + init + sib)
-
-        def leaf(row):                         # hash_rows: canonical words, 8 bytes little-endian each
-            return hashlib.sha256(b"".join((int(w) * _RINV % P).to_bytes(8, "little") for w in row)).digest()
-
-        digests = [leaf(row) for row in rows[k:]]
-        if isinstance(nodes, tuple):            # split heap: the top heap, then each block's local heap
-            top, blocks = nodes
-            self.ctx.sync()                     # the last blocks' copies to host memory
-            path_nodes = []
-            for i in path:
-                b, j = heap_location(i, log_b)
-                path_nodes.append((top[j] if b is None else blocks[b, j]).tobytes())
-        else:
-            path_nodes = [d.tobytes() for d in self.ctx.gather_rows_rowmajor(nodes, 4, N, path)] if path else []
-        return rows[:k], MerkleView(path_nodes, digests[:len(init)], digests[len(init):], N.bit_length() - 1)
-
-    def _prove_streamed(self, r):
-        ctx, air, channel, lap = r.ctx, r.air, r.channel, r.lap
-        fq, n, log_n, log_b, N, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.N, r.nbase, r.next_
-        offsets = coset_offsets(log_n, log_b)
-
-        # ---- base trace commitment: coefficients stay, the LDE passes through one block buffer
-        host_base = self._base_columns(r)
-        base = self._lookup_base(r, host_base) if air.lookups or air.permutations else self._to_device(host_base)
-        del host_base                           # held no longer than `base`: see release_base_columns below
-        base_polys, base_blk = self._empty(nbase, n), self._empty(nbase, n)
-        ctx.ntt_batch_to(base, base_polys, FP, log_n, nbase, inverse=True)
-        heaps = r.host_heaps if r.host_heaps is not None else [None] * 3
-        base_nodes, base_root = self._commit_blocks(base_polys, base_blk, FP, nbase, log_n, log_b, offsets, heaps[0])
-        channel.commit_base_trace(base_root)
-        lap("base_trace_commitment")
-        challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
-        hints = air.gen_hints(challenges)
-
-        # ---- extension trace commitment
-        ext = self._extension_columns(r, challenges, hints, base)
-        check = self._keep_for_check(r, base, ext)
-        del base
-        ext_polys = ext_blk = ext_nodes = None
-        if ext is not None:
-            ext = check[1] if check else ext
-            ext_polys = self._empty(next_, n * fq)
-            ctx.ntt_batch_to(self._to_device(ext), ext_polys, fq, log_n, next_, inverse=True)
-            del ext
-            ext_blk = self._empty(next_, n * fq)
-            ext_nodes, ext_root = self._commit_blocks(ext_polys, ext_blk, fq, next_, log_n, log_b, offsets, heaps[1])
-            channel.commit_extension_trace(ext_root)
-        lap("extension_trace_commitment")
-        self._check(r, challenges, hints, check)
-        del check
-
-        def trace_block(h):
-            self._block(base_polys, base_blk, FP, nbase, log_n, h)
-            cols = [base_blk[c] for c in range(nbase)]
-            if next_:
-                self._block(ext_polys, ext_blk, fq, next_, log_n, h)
-                cols += [ext_blk[c] for c in range(next_)]
-            return cols
-
-        # ---- constraint evaluation, block by block: the blocks q < ce_blowup of the LDE are the ce domain
-        ce_blowup = air.ce_blowup_factor
-        log_ce = log_n + ce_blowup.bit_length() - 1
-        M = n * ce_blowup
-        composition_coeffs = [channel.public_coin.draw() for _ in range(air.num_composition_constraint_coeffs())]
-        prog = block_program(r.cached_air).bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
-        comp_evals = self._empty(M * fq)
-        is_fq = [False] * nbase + [True] * next_
-        for q, h in offsets[:ce_blowup]:
-            ctx.eval_constraints_ptrs(prog, comp_evals[q * n * fq:(q + 1) * n * fq], log_n, trace_block(h), is_fq, fq_field=fq,
-                                      offset=h, trace_bitrev=True, out_bitrev=True)
-        lap("constraint_eval")
-
-        # ---- composition trace: the bit-reversed ce-domain column -> coefficients -> ce_blowup columns
-        ctx.bit_reverse(comp_evals, fq, log_ce)
-        if r.host_heaps is not None:
-            # the size-M transform's temporary (as large as the column: 12 GiB at 2^25 rows) is the context's own
-            # allocation and cannot reuse blocks torch's allocator keeps cached from the trace and extension columns
-            torch.cuda.empty_cache()
-        ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
-        comp_polys = self._composition_columns(r, comp_evals)
-        del comp_evals                          # (when ce_blowup == 1, comp_polys is a view of it and keeps it)
-        ctx.set_option("drop_scratch", 1)       # the size-M transform's temporary: as large as the column itself
-        comp_blk = self._empty(ce_blowup, n * fq)
-        comp_nodes, comp_root = self._commit_blocks(comp_polys, comp_blk, fq, ce_blowup, log_n, log_b, offsets, heaps[-1])
-        channel.commit_composition_trace(comp_root)
-        lap("composition_trace_commitment")
-
-        # ---- DEEP composition polynomial: every block of the three matrices recomputed once more
-        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
-        deep_lde = self._empty(N * fq)
-        is_fq = [False] * nbase + [True] * (next_ + ce_blowup)
-        for q, h in offsets:
-            cols = trace_block(h)
-            self._block(comp_polys, comp_blk, fq, ce_blowup, log_n, h)
-            cols += [comp_blk[c] for c in range(ce_blowup)]
-            ctx.eval_constraints_ptrs(dprog, deep_lde[q * n * fq:(q + 1) * n * fq], log_n, cols, is_fq, fq_field=fq, offset=h,
-                                      trace_bitrev=True, out_bitrev=True)
-        del base_blk, ext_blk, comp_blk
-        lap("deep_composition")
-
-        layers = self._fri(r, deep_lde)
-
-        # ---- queries: rows and leaf digests from the coefficients, path nodes from the node heaps
-        positions = channel.get_fri_query_positions()
-        fri_proof = self._fri_queries(r, layers, positions)
-        base_rows, base_view = self._streamed_queries(base_polys, FP, nbase, base_nodes, log_n, log_b, positions)
-        comp_rows, comp_view = self._streamed_queries(comp_polys, fq, ce_blowup, comp_nodes, log_n, log_b, positions)
-        ext_rows, ext_view = (self._streamed_queries(ext_polys, fq, next_, ext_nodes, log_n, log_b, positions) if next_
-                              else (None, None))
-        queries = Queries(_canon_rows(base_rows, 1), _canon_rows(ext_rows, fq) if next_ else [], _canon_rows(comp_rows, fq),
+        fri_proof, opened = rows.open(layers, positions, mats)
+        (base_rows, base_view), (ext_rows, ext_view), (comp_rows, comp_view) = opened
+        queries = Queries(_canon_rows(base_rows, 1), _canon_rows(ext_rows, fq) if ext_m else [], _canon_rows(comp_rows, fq),
                           base_view, ext_view, comp_view)
         return self._finish(r, fri_proof, queries)
 
-    # ---- phases every driver shares (ShardedProver included)
+    # ---- phases the sequence and the layouts share (ShardedProver included)
     def _lookup_base(self, r, host_base):
         """the prover's own device copy of the base columns (the caller's trace, host or device, is never written) with the
         columns the AIR leaves to the package filled: every permutation's targets first, in declaration order, then every
@@ -810,19 +631,9 @@ class GpuProver:
             r.lap("lookup_multiplicities", since=t)
         return base
 
-    def _keep_for_check(self, r, base, ext):
-        """with validation: the natural-order base columns and the extension columns on the device (a host-built
-        extension matrix uploaded once, for the check and the commitment), kept until the check has run"""
-        if not r.validate:
-            return None
-        return base, None if ext is None else self._to_device(ext)
-
-    def _check(self, r, challenges, hints, check):
-        """Stark::validate_constraints at the reference's position (src/prover.rs:74-75)"""
-        if check is not None:
-            r.air._check_program = r.cached_air.check_program()      # compiled once per AIR and trace length
-            r.stark.validate_constraints(r.air, challenges, hints, check[0], check[1], r.ctx)
-            r.lap("validate_constraints")
+    def _device_base(self, r, host_base):
+        """the base columns on the device: the prover's own filled copy when the AIR has lookups or permutations"""
+        return self._lookup_base(r, host_base) if r.air.lookups or r.air.permutations else self._to_device(host_base)
 
     def _extension_columns(self, r, challenges, hints, base):
         """the trace's own builder first (device or host); without one, the columns the AIR declares, built on the device"""
@@ -841,13 +652,14 @@ class GpuProver:
             raise ProvingError(f"expected {r.next_} extension columns, got {num_ext}")
         return ext
 
-    def _composition_columns(self, r, comp_coeffs):
-        """the composition coefficients over the ce coset as ce_blowup columns, column i = coefficients = i mod ce_blowup"""
-        ce_blowup = r.air.ce_blowup_factor
-        if ce_blowup == 1:
-            return comp_coeffs.view(1, r.n * r.fq)
-        comp_polys = self._empty(ce_blowup, r.n * r.fq)
-        r.ctx.matrix_from_rows(comp_coeffs, comp_polys, r.fq, r.n, ce_blowup)
+    def _composition_columns(self, r, comp_evals):
+        """the natural-order ce-domain column `comp_evals` (transformed in place) as its coefficients over the ce coset in
+        ce_blowup columns, column i = coefficients = i mod ce_blowup"""
+        r.ctx.ntt_batch(comp_evals, r.fq, r.log_ce, 1, inverse=True, offset=GEN_MONT)
+        if r.ce_blowup == 1:
+            return comp_evals.view(1, r.n * r.fq)
+        comp_polys = self._empty(r.ce_blowup, r.n * r.fq)
+        r.ctx.matrix_from_rows(comp_evals, comp_polys, r.fq, r.n, r.ce_blowup)
         return comp_polys
 
     def _bind_deep(self, r, base_polys, ext_polys, comp_polys):
@@ -891,18 +703,6 @@ class GpuProver:
             dkeys, z_points, z_m, [_lift(v) for v in execution_trace_oods], [_lift(v) for v in composition_trace_oods],
             [_lift(v) for v in ex_alphas], [_lift(v) for v in co_alphas], _lift(d_alpha), _lift(d_beta),
             trace_arguments=trace_arguments))
-
-    def _fri(self, r, deep_lde):
-        """FRI layers (fri.rs:179-249), the remainder and the proof of work; returns the committed layers"""
-        log_ff = r.options.fri_folding_factor.bit_length() - 1
-        layers = []
-        cur, ln = deep_lde, r.log_N
-        for _ in range(r.options.fri_num_layers(r.N)):
-            layer, cur = self._fri_layer(r, cur, ln)
-            layers.append(layer)
-            ln -= log_ff
-        self._fri_tail(r, cur, ln)
-        return layers
 
     def _fri_layer(self, r, cur, ln):
         """one FRI layer of the whole codeword `cur` (2^ln entries): commit its rows of ff entries, draw alpha, fold.
@@ -956,3 +756,227 @@ class GpuProver:
         c = r.channel
         return Proof(r.options, r.n, c.base_trace_commitment, c.extension_trace_commitment, c.composition_trace_commitment,
                      fri_proof, c.pow_nonce, queries, c.execution_trace_ood_evals, c.composition_trace_ood_evals, r.timings)
+
+
+class _Resident(_Layout):
+    """every LDE matrix and both arrays of every Merkle tree in HBM until the queries"""
+
+    def commit_base(self):
+        """A host trace is uploaded in column chunks on a second stream while the previous chunk is interpolated and
+        extended (columns are independent until the row hash); a pinned trace — the analogue of the reference's
+        GpuAllocator-backed columns — makes the copies asynchronous."""
+        p, r, ctx = self.p, self.r, self.p.ctx
+        n, N, nbase = r.n, r.N, r.nbase
+        host_base = p._base_columns(r)
+        if r.air.lookups or r.air.permutations or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
+            # the filled columns are written before the commitment, so the upload cannot overlap the transforms here
+            base = p._device_base(r, host_base)
+            return base, self.commit_evals([base], FP, nbase)
+        if not isinstance(host_base, torch.Tensor):
+            host_base = torch.from_numpy(np.ascontiguousarray(host_base, dtype=np.uint64).view(np.int64))
+        base, base_polys, base_lde = p._empty(nbase, n), p._empty(nbase, n), p._empty(nbase, N)
+        chunk = max(1, min(nbase, (64 << 20) // (8 * n) or 1))            # ~64 MiB per copy
+        p.copy_stream.wait_stream(p.stream)
+        events = []
+        with torch.cuda.stream(p.copy_stream):
+            for c0 in range(0, nbase, chunk):
+                c1 = min(c0 + chunk, nbase)
+                base[c0:c1].copy_(host_base[c0:c1], non_blocking=True)
+                ev = torch.cuda.Event()
+                ev.record(p.copy_stream)
+                events.append((c0, c1, ev))
+        for c0, c1, ev in events:
+            p.stream.wait_event(ev)
+            ctx.ntt_batch_to(base[c0], base_polys[c0], FP, r.log_n, c1 - c0, inverse=True)
+            ctx.lde_batch(base_polys[c0], base_lde[c0], FP, r.log_n, r.log_b, c1 - c0, offset=GEN_MONT, bitrev=True)
+        leaves, nodes = p._empty(N, 4), p._empty(N, 4)
+        root = ctx.merkle_commit(base_lde, FP, N, nbase, leaves=leaves, nodes=nodes)
+        return base, _Matrix(base_polys, base_lde, FP, nbase, _Tree(leaves, nodes, N), root)
+
+    def commit_evals(self, held, field, ncols):
+        """Matrix::interpolate over the trace domain, then commit_coeffs"""
+        evals = self.p._to_device(held[0])
+        polys = self.p._empty(ncols, self.r.n * field)
+        self.p.ctx.ntt_batch_to(evals, polys, field, self.r.log_n, ncols, inverse=True)
+        return self.commit_coeffs(polys, field, ncols)
+
+    def commit_coeffs(self, polys, field, ncols):
+        """bit-reversed LDE + Merkle commit of a column-major coefficient matrix"""
+        p, N = self.p, self.r.N
+        lde = p._empty(ncols, N * field)
+        p.ctx.lde_batch(polys, lde, field, self.r.log_n, self.r.log_b, ncols, offset=GEN_MONT, bitrev=True)
+        leaves, nodes = p._empty(N, 4), p._empty(N, 4)
+        root = p.ctx.merkle_commit(lde, field, N, ncols, leaves=leaves, nodes=nodes)
+        return _Matrix(polys, lde, field, ncols, _Tree(leaves, nodes, N), root)
+
+    def constraint_evals(self, base, ext, bind):
+        """The first M entries of a bit-reversed LDE column ARE the ce-coset evaluations in bit-reversed order, so they
+        are read in place (trace_bitrev); the output is in natural order"""
+        r = self.r
+        prog = r.air.composition_program().bind(**bind)
+        comp_evals = self.p._empty(r.n * r.ce_blowup * r.fq)
+        self.p.ctx.eval_constraints(prog, comp_evals, r.log_ce, base_cols=base.rows, nbase=r.nbase, base_stride=r.N,
+                                    ext_cols=ext.rows if ext else None, next_=r.next_, ext_stride=r.N, fq_field=r.fq,
+                                    offset=GEN_MONT, trace_bitrev=True)
+        return comp_evals
+
+    def composition_polys(self, held):
+        return self.p._composition_columns(self.r, held[0])
+
+    def deep_codeword(self, dprog, mats):
+        r = self.r
+        cols = [m.rows.data_ptr() + c * r.N * 8 * m.field for m in mats if m for c in range(m.ncols)]
+        codeword = self.p._empty(r.N * r.fq)
+        self.p.ctx.eval_constraints_ptrs(dprog, codeword, r.log_N, cols, [False] * r.nbase + [True] * (len(cols) - r.nbase),
+                                         fq_field=r.fq, offset=GEN_MONT, trace_bitrev=True, out_bitrev=True)
+        return codeword
+
+    def open(self, layers, positions, mats):
+        p, r = self.p, self.r
+        fri_proof = p._fri_queries(r, layers, positions)
+        rows = [p.ctx.gather_rows(m.rows, m.field, r.N, m.ncols, positions) if m else None for m in mats]
+        views = [p._view(m.tree, positions) if m else None for m in mats]
+        return fri_proof, list(zip(rows, views))
+
+
+class _Blocks(_Layout):
+    """a layout that evaluates coset block by coset block with the block-local program: self.blocks lists the (q, h_q)
+    it evaluates, block j at entries [j n, (j+1) n) of its codeword, and self._cols(j, h_q, mats) gives block j's columns"""
+
+    def constraint_evals(self, base, ext, bind):
+        """the blocks q < ce_blowup of the LDE are the ce domain; the column comes out bit-reversed"""
+        r = self.r
+        n, fq = r.n, r.fq
+        prog = block_program(r.cached_air).bind(**bind)
+        comp_evals = self.p._empty(n * r.ce_blowup * fq)
+        is_fq = [False] * r.nbase + [True] * r.next_
+        for j, (q, h) in enumerate(self.blocks):
+            if q < r.ce_blowup:
+                self.p.ctx.eval_constraints_ptrs(prog, comp_evals[q * n * fq:(q + 1) * n * fq], r.log_n,
+                                                 self._cols(j, h, (base, ext)), is_fq, fq_field=fq, offset=h,
+                                                 trace_bitrev=True, out_bitrev=True)
+        return comp_evals
+
+    def deep_codeword(self, dprog, mats):
+        r = self.r
+        n, fq = r.n, r.fq
+        codeword = self.p._empty(len(self.blocks) * n * fq)
+        is_fq = [False] * r.nbase + [True] * (r.next_ + r.ce_blowup)
+        for j, (q, h) in enumerate(self.blocks):
+            self.p.ctx.eval_constraints_ptrs(dprog, codeword[j * n * fq:(j + 1) * n * fq], r.log_n, self._cols(j, h, mats),
+                                             is_fq, fq_field=fq, offset=h, trace_bitrev=True, out_bitrev=True)
+        return codeword
+
+
+class _Streamed(_Blocks):
+    """only the coefficients and the tree nodes stay; each coset block of the LDE is recomputed into one block buffer
+    per matrix where it is needed, and query rows come from the coefficients.  host_heaps ((ntrees, beta, n, 32) bytes
+    of pinned host memory, streamed_host): the node heaps of the trees, in commitment order"""
+
+    def __init__(self, prover, r, host_heaps):
+        super().__init__(prover, r)
+        self.blocks = coset_offsets(r.log_n, r.log_b)
+        self.host_heaps = host_heaps
+        self.heaps = iter([None] * 3 if host_heaps is None else host_heaps)
+
+    def commit_base(self):
+        base = self.p._device_base(self.r, self.p._base_columns(self.r))
+        return base, self.commit_evals([base], FP, self.r.nbase)
+
+    def commit_evals(self, held, field, ncols):
+        evals = held.pop()
+        polys = self.p._empty(ncols, self.r.n * field)
+        self.p.ctx.ntt_batch_to(self.p._to_device(evals), polys, field, self.r.log_n, ncols, inverse=True)
+        del evals
+        return self.commit_coeffs(polys, field, ncols)
+
+    def commit_coeffs(self, polys, field, ncols):
+        """Merkle commitment of the bit-reversed LDE, one coset block at a time: block q is transformed into the block
+        buffer and hashed into its subtree of the node heap; the top log_b levels come from the block roots.  With a host
+        heap ((beta, n, 32) bytes), block q's subtree is its local heap host_heap[q] and the tree is (top heap of 2 beta
+        digests on the host, host_heap): the split layout of include/ministark_host_nodes.h."""
+        ctx, r = self.p.ctx, self.r
+        beta, host_heap = r.beta, next(self.heaps)
+        m = _Matrix(polys, self.p._empty(ncols, r.n * field), field, ncols)
+        if host_heap is None:
+            nodes, roots = self.p._empty(beta << r.log_n, 4), self.p._empty(beta, 4)
+        else:
+            nodes = self.p._empty(2 * beta, 4)
+            roots = nodes[beta:]
+        for q, h in self.blocks:
+            self._block(m, h)
+            if host_heap is None:
+                ctx.merkle_commit_block(m.rows, field, r.log_n, r.log_b, q, ncols, nodes, roots[q])
+            else:
+                ctx.merkle_commit_block_host(m.rows, field, r.log_n, ncols, host_heap[q], roots[q])
+        if beta > 1:
+            ctx.merkle_nodes(roots, nodes, beta)
+        nodes[0].zero_()                        # the unused default digest (named by a walk over a 2-leaf tree)
+        m.root = nodes[1].cpu().numpy().tobytes()
+        m.tree = nodes if host_heap is None else (nodes.cpu().numpy().view(np.uint8), host_heap)
+        return m
+
+    def _block(self, m, h):
+        """coset block with offset h of the bit-reversed LDE of every column of `m`, into its block buffer.  Its NTT plan
+        is dropped at once: every block has its own offset, and beta cached plans with their full tables (up to GiBs each
+        at 2^24 points) would take back the memory streaming saves"""
+        self.p.ctx.lde_batch(m.polys, m.rows, m.field, self.r.log_n, 0, m.ncols, offset=h, bitrev=True)
+        self.p.ctx.set_option("drop_plans", 1)
+
+    def _cols(self, j, h, mats):
+        """block j (offset h) of every column of `mats`, recomputed into their block buffers"""
+        cols = []
+        for m in mats:
+            if m:
+                self._block(m, h)
+                cols += [m.rows[c] for c in range(m.ncols)]
+        return cols
+
+    def composition_polys(self, held):
+        ctx, r = self.p.ctx, self.r
+        comp_evals = held.pop()
+        ctx.bit_reverse(comp_evals, r.fq, r.log_ce)
+        if self.host_heaps is not None:
+            # the size-M transform's temporary (as large as the column: 12 GiB at 2^25 rows) is the context's own
+            # allocation and cannot reuse blocks torch's allocator keeps cached from the trace and extension columns
+            torch.cuda.empty_cache()
+        comp_polys = self.p._composition_columns(r, comp_evals)
+        del comp_evals                          # (when ce_blowup == 1, comp_polys is a view of it and keeps it)
+        ctx.set_option("drop_scratch", 1)       # the size-M transform's temporary: as large as the column itself
+        return comp_polys
+
+    def deep_codeword(self, dprog, mats):
+        """every block of the three matrices recomputed once more; the block buffers are released afterwards"""
+        codeword = super().deep_codeword(dprog, mats)
+        for m in mats:
+            if m:
+                m.rows = None
+        return codeword
+
+    def open(self, layers, positions, mats):
+        fri_proof = self.p._fri_queries(self.r, layers, positions)
+        opened = {k: self._query(mats[k], positions) for k in (0, 2, 1) if mats[k]}      # base, composition, extension
+        return fri_proof, [opened.get(k, (None, None)) for k in range(3)]
+
+    def _query(self, m, positions):
+        """the rows at `positions` and their MerkleView without the LDE: rows and leaf digests from the coefficients
+        (ms_lde_rows), path nodes gathered from the node heap"""
+        ctx, r = self.p.ctx, self.r
+        init, sib, path = merkle_walk(r.N, positions)
+        k = len(positions)
+        rows = ctx.lde_rows(m.polys, m.field, r.log_n, r.log_b, m.ncols, list(positions) + init + sib)
+
+        def leaf(row):                         # hash_rows: canonical words, 8 bytes little-endian each
+            return hashlib.sha256(b"".join((int(w) * _RINV % P).to_bytes(8, "little") for w in row)).digest()
+
+        digests = [leaf(row) for row in rows[k:]]
+        if isinstance(m.tree, tuple):           # split heap: the top heap, then each block's local heap
+            top, blocks = m.tree
+            ctx.sync()                          # the last blocks' copies to host memory
+            path_nodes = []
+            for i in path:
+                b, j = heap_location(i, r.log_b)
+                path_nodes.append((top[j] if b is None else blocks[b, j]).tobytes())
+        else:
+            path_nodes = [d.tobytes() for d in ctx.gather_rows_rowmajor(m.tree, 4, r.N, path)] if path else []
+        return rows[:k], MerkleView(path_nodes, digests[:len(init)], digests[len(init):], r.N.bit_length() - 1)

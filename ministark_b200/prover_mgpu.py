@@ -23,23 +23,21 @@ proof bytes are identical to the single-GPU prover's (tests/test_gpu_multi.py), 
 A FRI layer is sharded while every rank still holds at least two of its rows; the remaining small layers are gathered
 once and finished on every rank.  torch / torch.distributed are plumbing: buffers, the stream, the collectives.
 
-ShardedProver is a GpuProver: only what depends on where the LDE rows live is written here (the column-split
-interpolation, the slab LDE and commitment, the block-wise constraint evaluation and DEEP, the sharded FRI layers and
-the query fetch plan).  The set-up, the phase clock, the base-column read, the permutation and lookup fills, the
-extension and composition columns, the OOD/DEEP binding, the gathered FRI layers, the remainder and proof of work, and
-the proof assembly are GpuProver's methods, shared with its resident and streamed drivers.
+ShardedProver is a GpuProver that runs GpuProver._default_prove with the _Sharded layout: only what depends on where
+the LDE rows live is written here (the column-split interpolation, the slab LDE and commitment, the broadcast of the
+ce-domain column, the sharded FRI layers and the query fetch plan).
 """
 import hashlib
 
 import numpy as np
 import torch
 
-from . import FP, GENERATOR as GEN_MONT
+from . import FP
 from . import expr as E
 from .air import domain_generator
-from .cosets import block_program, brev as _brev, coset_offsets, merkle_walk
-from .proof import LayerProof, MerkleView, Queries
-from .prover import GpuProver, ProvingError, _Run, _canon_rows, _lift, _mont
+from .cosets import brev as _brev, coset_offsets, merkle_walk
+from .proof import LayerProof, MerkleView
+from .prover import GpuProver, ProvingError, _Blocks, _Matrix, _Run, _canon_rows, _lift, _mont
 
 P = E.P
 _R = 2**64
@@ -284,127 +282,93 @@ class ShardedProver(GpuProver):
             cur = full
         return layers, gathered, cur, ln
 
-    # ---- default_prove: the set-up and every phase that does not depend on where the LDE rows live are GpuProver's
+    # ---- default_prove: GpuProver's sequence, with this rank's slab of every matrix
     def _prove(self, stark, options, witness, validate=False):
         if validate:
             raise ProvingError("the sharded prover does not validate the trace (its ranks need not hold the whole base "
                                "trace): validate with GpuProver")
         r = self._start(stark, options, witness, False)
-        ctx, dist, G = self.ctx, self.dist, self.world
-        air, channel, lap = r.air, r.channel, r.lap
-        fq, n, log_n, log_b, nbase, next_ = r.fq, r.n, r.log_n, r.log_b, r.nbase, r.next_
-        if r.beta % G or n < 16:
+        if r.beta % self.world or r.n < 16:
             raise ProvingError("the sharded prover needs a world size dividing the LDE blow-up factor and n >= 16")
-        bpr, rows_per = r.beta // G, r.N // G
-        my_blocks = self._offsets(log_n, log_b)
-        lap("init_air")
+        r.lap("init_air")
+        return self._default_prove(r, _Sharded(self, r))
 
-        # ---- base trace commitment (prover.rs:46-55)
-        host_base = self._base_columns(r)
-        needs_full_base = next_ > 0          # extension columns are built from the whole base trace (on every rank)
-        if needs_full_base or nbase < G or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
-            # with lookups or permutations every rank fills its own copy (each has an extension column)
-            base = self._lookup_base(r, host_base) if air.lookups or air.permutations else self._to_device(host_base)
-            base_polys = self._interpolate(base, FP, nbase, log_n)
+
+class _Sharded(_Blocks):
+    """this rank's blocks of every matrix: a slab of N/G consecutive rows of the bit-reversed LDE, committed as this
+    rank's subtree of the global tree"""
+
+    def __init__(self, prover, r):
+        super().__init__(prover, r)
+        self.blocks = prover._offsets(r.log_n, r.log_b)
+        self.rows_per = r.N // prover.world
+
+    def commit_base(self):
+        p, r = self.p, self.r
+        host_base = p._base_columns(r)
+        # extension columns are built from the whole base trace (on every rank); with lookups or permutations every
+        # rank fills its own copy (each has an extension column)
+        if r.next_ > 0 or r.nbase < p.world or (isinstance(host_base, torch.Tensor) and host_base.is_cuda):
+            base = p._device_base(r, host_base)
+            polys = p._interpolate(base, FP, r.nbase, r.log_n)
         else:
-            base = None
-            base_polys = self._interpolate(host_base, FP, nbase, log_n, from_host=True)
+            base, polys = None, p._interpolate(host_base, FP, r.nbase, r.log_n, from_host=True)
         del host_base
-        base_slab = self._lde_slab(base_polys, FP, nbase, log_n, log_b)
-        base_tree, base_root = self._commit_slab(base_slab, FP, nbase, rows_per)
-        channel.commit_base_trace(base_root)
-        lap("base_trace_commitment")
-        challenges = [channel.public_coin.draw() for _ in range(air.num_challenges())]
-        hints = air.gen_hints(challenges)
+        return base, self.commit_coeffs(polys, FP, r.nbase)
 
-        # ---- extension trace commitment (prover.rs:56-72): built from the (replicated) base trace on every rank
-        ext = self._extension_columns(r, challenges, hints, base)
-        del base
-        ext_polys = ext_slab = ext_tree = None
-        if ext is not None:
-            ext_polys = self._interpolate(self._to_device(ext), fq, next_, log_n)
-            ext_slab = self._lde_slab(ext_polys, fq, next_, log_n, log_b)
-            ext_tree, ext_root = self._commit_slab(ext_slab, fq, next_, rows_per)
-            channel.commit_extension_trace(ext_root)
-        del ext
-        lap("extension_trace_commitment")
+    def commit_evals(self, held, field, ncols):
+        return self.commit_coeffs(self.p._interpolate(self.p._to_device(held[0]), field, ncols, self.r.log_n), field, ncols)
 
-        # ---- constraint evaluation (prover.rs:75-108), block by block: the blocks q < ce_blowup of the LDE are the ce
-        # domain; each is evaluated where it lives, then the (small) evaluation column is shared
-        ce_blowup = air.ce_blowup_factor
-        log_ce = log_n + ce_blowup.bit_length() - 1
-        M = n * ce_blowup
-        composition_coeffs = [channel.public_coin.draw() for _ in range(air.num_composition_constraint_coeffs())]
-        prog = block_program(r.cached_air).bind(challenges=challenges, hints=hints, ccoefs=composition_coeffs)
-        comp_evals = self._empty(M * fq)
-        is_fq = [False] * nbase + [True] * next_
-        for j, (q, h) in enumerate(my_blocks):
-            if q < ce_blowup:
-                cols = self._block_ptrs(base_slab, FP, nbase, rows_per, j, n)
-                if next_:
-                    cols += self._block_ptrs(ext_slab, fq, next_, rows_per, j, n)
-                ctx.eval_constraints_ptrs(prog, comp_evals[q * n * fq:(q + 1) * n * fq], log_n, cols, is_fq, fq_field=fq,
-                                          offset=h, trace_bitrev=True, out_bitrev=True)
-        for q in range(ce_blowup):
-            dist.broadcast(comp_evals[q * n * fq:(q + 1) * n * fq], src=q // bpr)
-        lap("constraint_eval")
+    def commit_coeffs(self, polys, field, ncols):
+        slab = self.p._lde_slab(polys, field, ncols, self.r.log_n, self.r.log_b)
+        tree, root = self.p._commit_slab(slab, field, ncols, self.rows_per)
+        return _Matrix(polys, slab, field, ncols, tree, root)
 
-        # ---- composition trace (prover.rs:110-125): one column over the ce coset -> coefficients -> ce_blowup columns.
-        # comp_evals is the bit-reversed ce-domain column; one small transform, done on every rank
-        ctx.bit_reverse(comp_evals, fq, log_ce)
-        ctx.ntt_batch(comp_evals, fq, log_ce, 1, inverse=True, offset=GEN_MONT)
-        comp_polys = self._composition_columns(r, comp_evals)
-        comp_slab = self._lde_slab(comp_polys, fq, ce_blowup, log_n, log_b)
-        comp_tree, comp_root = self._commit_slab(comp_slab, fq, ce_blowup, rows_per)
-        channel.commit_composition_trace(comp_root)
-        lap("composition_trace_commitment")
+    def _cols(self, j, h, mats):
+        return [c for m in mats if m for c in self.p._block_ptrs(m.rows, m.field, m.ncols, self.rows_per, j, self.r.n)]
 
-        # ---- DEEP composition polynomial over this rank's LDE rows (composer.rs:89-188 in evaluation form), bound from
-        # the out-of-domain evaluations of the replicated coefficients
-        dprog = self._bind_deep(r, base_polys, ext_polys, comp_polys)
-        ncols_all = nbase + next_ + ce_blowup
-        deep_slab = self._empty(rows_per * fq)
-        for j, (q, h) in enumerate(my_blocks):
-            cols = self._block_ptrs(base_slab, FP, nbase, rows_per, j, n)
-            if next_:
-                cols += self._block_ptrs(ext_slab, fq, next_, rows_per, j, n)
-            cols += self._block_ptrs(comp_slab, fq, ce_blowup, rows_per, j, n)
-            ctx.eval_constraints_ptrs(dprog, deep_slab[j * n * fq:(j + 1) * n * fq], log_n, cols,
-                                      [False] * nbase + [True] * (ncols_all - nbase), fq_field=fq, offset=h,
-                                      trace_bitrev=True, out_bitrev=True)
-        lap("deep_composition")
+    def constraint_evals(self, base, ext, bind):
+        """each block is evaluated where it lives, then the (small) evaluation column is shared"""
+        comp_evals = super().constraint_evals(base, ext, bind)
+        n, fq = self.r.n, self.r.fq
+        for q in range(self.r.ce_blowup):
+            self.p.dist.broadcast(comp_evals[q * n * fq:(q + 1) * n * fq], src=q // (self.r.beta // self.p.world))
+        return comp_evals
 
-        # ---- FRI (fri.rs:179-249): layers sharded by rows while every rank keeps >= 2 rows of the layer
-        layers, gathered, cur, ln = self.fri_commit(deep_slab, r.log_N, fq, options, channel)
-        self._fri_tail(r, cur, ln)
+    def composition_polys(self, held):
+        """one small transform of the whole ce-domain column, done on every rank"""
+        self.p.ctx.bit_reverse(held[0], self.r.fq, self.r.log_ce)
+        return self.p._composition_columns(self.r, held[0])
 
-        # ---- queries (fri.rs:151-177, trace.rs:115-157): rows and path digests come from the ranks that own them
-        ff = options.fri_folding_factor
-        positions = channel.get_fri_query_positions()
+    def fri(self, codeword):
+        """layers sharded by rows while every rank keeps >= 2 rows of the layer, then gathered"""
+        layers, gathered, cur, ln = self.p.fri_commit(codeword, self.r.log_N, self.r.fq, self.r.options, self.r.channel)
+        self.p._fri_tail(self.r, cur, ln)
+        return layers, gathered
+
+    def open(self, layers, positions, mats):
+        """rows and path digests come from the ranks that own them"""
+        p, r, ctx = self.p, self.r, self.p.ctx
+        layers, gathered = layers
+        ff, fq, rows_per = r.options.fri_folding_factor, r.fq, self.rows_per
         pos_sorted = sorted(set(positions))
-        plan = _FetchPlan(self)
+        plan = _FetchPlan(p)
         pending, folded = [], positions
         for evals, tree, root, nrows in layers:
-            folded = sorted(set(p // ff for p in folded))
-            nloc = nrows // G
+            folded = sorted(set(q // ff for q in folded))
+            nloc = nrows // p.world
             hr = plan.rows(lambda loc, e=evals, k=nloc: ctx.gather_rows_rowmajor(e, ff * fq, k, loc), nloc, folded, ff * fq)
             pending.append((root, hr, plan.view(tree, folded)))
 
-        def trace_rows(slab, field, ncols):
+        def trace_rows(m):
             # Queries::new keeps the caller's position order (sorted, deduplicated by draw_queries)
-            return plan.rows(lambda loc: ctx.gather_rows(slab, field, rows_per, ncols, loc, col_stride=rows_per), rows_per, positions,
-                             ncols * field)
+            return plan.rows(lambda loc: ctx.gather_rows(m.rows, m.field, rows_per, m.ncols, loc, col_stride=rows_per),
+                             rows_per, positions, m.ncols * m.field)
 
-        h_base, h_comp = trace_rows(base_slab, FP, nbase), trace_rows(comp_slab, fq, ce_blowup)
-        h_ext = trace_rows(ext_slab, fq, next_) if next_ else None
-        v_base, v_comp = plan.view(base_tree, pos_sorted), plan.view(comp_tree, pos_sorted)
-        v_ext = plan.view(ext_tree, pos_sorted) if next_ else None
+        order = [k for k in (0, 2, 1) if mats[k]]          # base, composition, extension
+        handles = {k: trace_rows(mats[k]) for k in order}
+        views = {k: plan.view(mats[k].tree, pos_sorted) for k in order}
         plan.execute()
-        fri_proof = self._fri_queries(r, gathered, folded)      # the gathered layers: on every rank
+        fri_proof = p._fri_queries(r, gathered, folded)      # the gathered layers: on every rank
         fri_proof.layers[:0] = [LayerProof(_canon_rows(plan.get_rows(hr), fq), plan.get_view(hv), root) for root, hr, hv in pending]
-        queries = Queries(
-            _canon_rows(plan.get_rows(h_base), 1),
-            _canon_rows(plan.get_rows(h_ext), fq) if next_ else [],
-            _canon_rows(plan.get_rows(h_comp), fq),
-            plan.get_view(v_base), plan.get_view(v_ext) if next_ else None, plan.get_view(v_comp))
-        return self._finish(r, fri_proof, queries)
+        return fri_proof, [(plan.get_rows(handles[k]), plan.get_view(views[k])) if mats[k] else (None, None) for k in range(3)]
