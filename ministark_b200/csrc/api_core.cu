@@ -177,9 +177,12 @@ int ms_ctx_create(int device, ms_ctx **out) {
             a = gl::mul(a, w);
             b = gl::mul(b, wi);
         }
+        // on the context's own stream and waited for: a synchronous copy from pageable memory may return before its
+        // DMA lands, and this context's kernels run on a non-blocking stream
         u64 *d = nullptr;
         if (cudaMalloc(&d, h.size() * 8) != cudaSuccess ||
-            cudaMemcpy(d, h.data(), h.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaMemcpyAsync(d, h.data(), h.size() * 8, cudaMemcpyHostToDevice, c->own_stream) != cudaSuccess ||
+            cudaStreamSynchronize(c->own_stream) != cudaSuccess) {
             delete c;
             return MS_ERR_CUDA;
         }

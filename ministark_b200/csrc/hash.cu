@@ -229,11 +229,10 @@ __global__ void gather_digests_kernel(const uint4 *__restrict__ leaves, const ui
 // MS_SHA_FMA_ADDS=0 keeps every addition on the ALU pipe (the compiler's choice); the default mask 7 moves the
 // schedule and round-function additions to the FMA pipe (profiles/exp_sha.py times a mask against another).
 static int sha_variant() {
-    static int v = -1;
-    if (v < 0) {
+    static const int v = [] {
         const char *e = getenv("MS_SHA_FMA_ADDS");
-        v = (e && atoi(e) == 0) ? 0 : 7;
-    }
+        return (e && atoi(e) == 0) ? 0 : 7;
+    }();
     return v;
 }
 #define MS_SHA_DISPATCH(KERNEL, GRID, ...)                                        \
@@ -266,7 +265,10 @@ static int upload_pad_schedule(ms_ctx *c) {
     if (dev >= 0 && dev < 64 && done[dev]) return MS_OK;
     u32 kw[64];
     pad_schedule(512, kw);
-    MS_CUDA(c, cudaMemcpyToSymbol(c_KW_pad64, kw, sizeof kw));
+    // complete before `done` is set: a synchronous copy from pageable memory may return before its DMA lands, and the
+    // kernels of other contexts (other streams, other threads) read the constant as soon as `done` says so
+    MS_CUDA(c, cudaMemcpyToSymbolAsync(c_KW_pad64, kw, sizeof kw, 0, cudaMemcpyHostToDevice, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
     if (dev >= 0 && dev < 64) done[dev] = true;
     return MS_OK;
 }
