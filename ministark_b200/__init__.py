@@ -435,6 +435,17 @@ class Context:
         row-major, host or device; ms_rescue_hash); not synchronised"""
         self._ck(self.lib.ms_rescue_hash(self.h, _ptr(messages), int(K), int(length), _ptr(out)))
 
+    # ---- examples/merkle tree and paths (include/ministark_rescue_merkle.h)
+    def rescue_merkle_tree(self, leaves, depth, nodes):
+        """write `nodes`, the (2^(D + 1), 4) heap of the Rescue-Prime Merkle tree over `leaves` ((2^D, 4) canonical
+        words, host or device; ms_rescue_merkle_tree); not synchronised when both are device memory"""
+        self._ck(self.lib.ms_rescue_merkle_tree(self.h, _ptr(leaves), int(depth), _ptr(nodes)))
+
+    def rescue_merkle_paths(self, nodes, depth, indices, K, out):
+        """write `out`, the (14, 8 K L) trace of the K authentication paths of `indices` (K uint64 words, host or
+        device) through the heap `nodes` of depth D (host or device; ms_rescue_merkle_paths); synchronises"""
+        self._ck(self.lib.ms_rescue_merkle_paths(self.h, _ptr(nodes), int(depth), _ptr(indices), int(K), _ptr(out)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

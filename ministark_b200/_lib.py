@@ -20,6 +20,7 @@ DEVICE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_
 HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_host_nodes.h")
 RESCUE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue.h")
 RESCUE_HASH_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_hash.h")
+RESCUE_MERKLE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -131,6 +132,12 @@ _RESCUE_HASH_SIGS = {
     "ms_rescue_hash": (ci, [vp, vp, u64, u64, vp]),
 }
 
+# include/ministark_rescue_merkle.h: examples/merkle's Rescue-Prime Merkle tree and authentication-path trace
+_RESCUE_MERKLE_SIGS = {
+    "ms_rescue_merkle_tree": (ci, [vp, vp, ui, vp]),
+    "ms_rescue_merkle_paths": (ci, [vp, vp, ui, vp, u64, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -168,6 +175,7 @@ def load():
         bind(lib, _HOST_NODES_SIGS)
         bind(lib, _RESCUE_SIGS)
         bind(lib, _RESCUE_HASH_SIGS)
+        bind(lib, _RESCUE_MERKLE_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -487,8 +487,9 @@ class RescueAirConfig(AirConfig):
 
 def digest_evaluation(digests, gamma):
     """R's value on the last row: acc <- acc gamma^4 + d_0 + gamma d_1 + gamma^2 d_2 + gamma^3 d_3 over the chains in
-    order, from acc = 0 (gamma: a 3-tuple)"""
-    # that is sum_j a_j gamma^j with a_(4 (K - 1 - k) + w) = word w of digest k, evaluated in blocks of `block`
+    order, from acc = 0 (gamma: a 3-tuple).  Any tuple width W works the same way, acc <- acc gamma^W + sum_w gamma^w
+    d_w, as long as every tuple has W words (examples/merkle binds 5-word tuples)."""
+    # that is sum_j a_j gamma^j with a_(W (K - 1 - k) + w) = word w of tuple k, evaluated in blocks of `block`
     # coefficients: inside a block a dot product of base-field words with gamma^0 .. gamma^(block - 1), one component at
     # a time; across blocks Horner steps by gamma^block (about 25 times faster than one Fq3 product per word)
     gamma = E._q(gamma)
