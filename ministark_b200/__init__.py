@@ -446,6 +446,14 @@ class Context:
         device) through the heap `nodes` of depth D (host or device; ms_rescue_merkle_paths); synchronises"""
         self._ck(self.lib.ms_rescue_merkle_paths(self.h, _ptr(nodes), int(depth), _ptr(indices), int(K), _ptr(out)))
 
+    def rescue_merkle_updates(self, nodes, depth, indices, new_leaves, K, out, roots):
+        """apply K leaf writes in order to the heap `nodes` of depth D, in place: leaf indices[k] (K uint64 words) becomes
+        new_leaves[k] ((K, 4) canonical words); write `out`, the (15, 16 K L) trace of the old and the new paths, and
+        `roots`, the (K + 1, 4) roots before the first write and after each (all host or device;
+        ms_rescue_merkle_updates); synchronises"""
+        self._ck(self.lib.ms_rescue_merkle_updates(self.h, _ptr(nodes), int(depth), _ptr(indices), _ptr(new_leaves),
+                                                   int(K), _ptr(out), _ptr(roots)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

@@ -21,6 +21,7 @@ HOST_NODES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "minist
 RESCUE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue.h")
 RESCUE_HASH_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_hash.h")
 RESCUE_MERKLE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle.h")
+RESCUE_MERKLE_UPDATES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle_updates.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -138,6 +139,11 @@ _RESCUE_MERKLE_SIGS = {
     "ms_rescue_merkle_paths": (ci, [vp, vp, ui, vp, u64, vp]),
 }
 
+# include/ministark_rescue_merkle_updates.h: the trace of examples/merkle's K ordered leaf writes, and the heap after them
+_RESCUE_MERKLE_UPDATES_SIGS = {
+    "ms_rescue_merkle_updates": (ci, [vp, vp, ui, vp, vp, u64, vp, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -176,6 +182,7 @@ def load():
         bind(lib, _RESCUE_SIGS)
         bind(lib, _RESCUE_HASH_SIGS)
         bind(lib, _RESCUE_MERKLE_SIGS)
+        bind(lib, _RESCUE_MERKLE_UPDATES_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

@@ -1,7 +1,7 @@
 // rescue.cu — the traces of examples/rescue and examples/merkle, side by side on the device: K independent chains of L
 // Rescue-Prime permutations (include/ministark_rescue.h), K messages absorbed by the Rescue-Prime sponge
-// (include/ministark_rescue_hash.h), and the Rescue-Prime Merkle tree with K authentication paths through it
-// (include/ministark_rescue_merkle.h).
+// (include/ministark_rescue_hash.h), the Rescue-Prime Merkle tree with K authentication paths through it
+// (include/ministark_rescue_merkle.h), and K ordered leaf writes into that tree (include/ministark_rescue_merkle_updates.h).
 //
 // One chain (or message, tree node, path) per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's
 // parameters and write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the
@@ -13,8 +13,11 @@
 #include "../../include/ministark_rescue.h"
 #include "../../include/ministark_rescue_hash.h"
 #include "../../include/ministark_rescue_merkle.h"
+#include "../../include/ministark_rescue_merkle_updates.h"
 #include "ctx.cuh"
 #include "rescue_params.cuh"
+
+#include <cub/cub.cuh>
 
 namespace ms {
 
@@ -231,8 +234,173 @@ __global__ void __launch_bounds__(kThreads) rescue_merkle_paths_kernel(PathArgs 
     }
 }
 
+// ------------------------------------------------------------------------------- examples/merkle: ordered writes
+// Level j of K writes: write k passes node v_k = (2^D + i_k) >> j, side b_k = bit j of i_k, parent v_k >> 1.  Sorting
+// the writes stably by parent puts both children of a parent in one run, in write order.  Within a run, the sibling
+// write k sees is the new value of the latest earlier entry on the other side, and (level 0) the leaf it replaces the
+// new value of the latest earlier entry on its own side; without one, the heap's.  Marks hold 1-based positions: an
+// inclusive max-scan of (run start, last side-0 entry, last side-1 entry) gives each, and an entry found before the
+// run start belongs to another run.
+struct UpdateMarks {
+    u32 start, last[2];
+};
+
+struct UpdateMarksMax {
+    __device__ __forceinline__ UpdateMarks operator()(const UpdateMarks &a, const UpdateMarks &b) const {
+        return {a.start > b.start ? a.start : b.start, {a.last[0] > b.last[0] ? a.last[0] : b.last[0],
+                                                        a.last[1] > b.last[1] ? a.last[1] : b.last[1]}};
+    }
+};
+
+constexpr unsigned kUpdateThreads = 256;
+
+// the indices below 2^D and the leaf words canonical (the first failing position of each, atomically), and the new
+// leaves in Montgomery form into cur (the new paths' level-0 inputs)
+__global__ void update_check_kernel(const u64 *indices, const u64 *leaves, u64 K, u64 bound, u64 *cur,
+                                    unsigned long long *first_bad) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < 4 * K; i += (u64)gridDim.x * blockDim.x) {
+        if (i < K && indices[i] >= bound) atomicMin(first_bad, (unsigned long long)i);
+        const u64 w = leaves[i];
+        if (w >= gl::P) atomicMin(first_bad + 1, (unsigned long long)i);
+        cur[i] = gl::to_mont(w < gl::P ? w : 0);
+    }
+}
+
+__global__ void update_keys_kernel(const u64 *indices, u64 K, unsigned shift, u32 *keys, u32 *vals) {
+    const u64 k = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (k >= K) return;
+    keys[k] = (u32)(indices[k] >> shift);
+    vals[k] = (u32)k;
+}
+
+__global__ void update_marks_kernel(const u32 *keys, const u32 *order, const u64 *indices, u64 K, unsigned j,
+                                    UpdateMarks *marks) {
+    const u64 t = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (t >= K) return;
+    const unsigned b = (indices[order[t]] >> j) & 1;
+    UpdateMarks m;
+    m.start = t == 0 || keys[t] != keys[t - 1] ? (u32)(t + 1) : 0;
+    m.last[0] = b ? 0 : (u32)(t + 1);
+    m.last[1] = b ? (u32)(t + 1) : 0;
+    marks[t] = m;
+}
+
+struct ResolveArgs {
+    const u64 *nodes;           // the original heap, canonical
+    const u64 *indices;
+    const u32 *order;           // sorted position -> write
+    const UpdateMarks *scan;    // inclusive max-scan of the marks
+    const u64 *cur_new;         // K x 4 Montgomery: each write's new value of its level-j node
+    u64 *sib;                   // K x 4 Montgomery: the sibling each write sees
+    u64 *cur_old;               // level 0 only: K x 4 Montgomery, the leaf each write replaces
+    unsigned char *last;        // K flags of level j: cleared for every write a later one in the same node follows
+    u64 K;
+    unsigned D, j;
+};
+
+__global__ void update_resolve_kernel(ResolveArgs a) {
+    const u64 t = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (t >= a.K) return;
+    const u32 k = a.order[t];
+    const u64 v = ((1ull << a.D) + a.indices[k]) >> a.j;
+    const unsigned b = v & 1;
+    const u32 start = a.scan[t].start;
+    const UpdateMarks before = t ? a.scan[t - 1] : UpdateMarks{0, {0, 0}};
+    const u32 other = b ? before.last[0] : before.last[1], same = b ? before.last[1] : before.last[0];
+    if (other >= start) {
+        const u32 k2 = a.order[other - 1];
+        for (int w = 0; w < 4; w++) a.sib[4 * (u64)k + w] = a.cur_new[4 * (u64)k2 + w];
+    } else {
+        for (int w = 0; w < 4; w++) a.sib[4 * (u64)k + w] = gl::to_mont(a.nodes[4 * (v ^ 1) + w]);
+    }
+    if (same >= start) a.last[a.order[same - 1]] = 0;
+    if (a.j == 0) {
+        if (same >= start) {
+            const u32 k2 = a.order[same - 1];
+            for (int w = 0; w < 4; w++) a.cur_old[4 * (u64)k + w] = a.cur_new[4 * (u64)k2 + w];
+        } else {
+            for (int w = 0; w < 4; w++) a.cur_old[4 * (u64)k + w] = gl::to_mont(a.nodes[4 * v + w]);
+        }
+    }
+}
+
+struct UpdateArgs {
+    const u64 *indices;
+    const u64 *cur_in[2];       // K x 4 Montgomery inputs of the old (0) and new (1) paths at this level
+    u64 *cur_out[2];            // their outputs, words 0..3: the inputs of the next level
+    const u64 *sib;             // K x 4 Montgomery siblings (nullptr on filler levels)
+    u64 *roots;                 // (K + 1) x 4 canonical, written at level D - 1
+    u64 K, L, n;
+    unsigned D, j;
+    u64 *out;
+};
+
+// one path per 16 lanes, the old (even group) and the new (odd group) path of one write side by side in a warp, path
+// g = 2 k + side at rows 8 (L g + j) + r: lanes 0..3 and 4..7 take the path's current node and the sibling in the order
+// bit j gives; lane 12 writes BIT, lane 13 IDX and lane 14 SIDE
+__global__ void __launch_bounds__(kThreads) rescue_merkle_update_kernel(UpdateArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 g = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool in_range = g < 2 * a.K, live = in_range && lane < (unsigned)kW;
+    const unsigned w = lane < (unsigned)kW ? lane : kW - 1;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+    load_params(w, row, c1, c2);
+    const u64 k = in_range ? g >> 1 : 0;
+    const unsigned side = g & 1;
+    const u64 idx = a.indices[k];
+    const bool bit = a.j < a.D && ((idx >> a.j) & 1);
+    u64 s = 0;
+    if (lane < 8) {
+        const u64 cur = (side ? a.cur_in[1] : a.cur_in[0])[4 * k + (lane & 3)];
+        const u64 sib = a.sib ? a.sib[4 * k + (lane & 3)] : 0;
+        s = (lane < 4) != bit ? cur : sib;
+    }
+    const u64 at = 8 * (a.L * (2 * k + side) + a.j);
+    u64 *col = a.out + (u64)w * a.n + at;
+#pragma unroll
+    for (int r = 0; r < kRounds; r++) {
+        if (live) col[r] = s;
+        s = rescue_round(row, c1[r], c2[r], s);
+    }
+    if (live) col[kRounds] = s;
+    if (in_range && lane < 4) {
+        (side ? a.cur_out[1] : a.cur_out[0])[4 * k + lane] = s;
+        if (a.j + 1 == a.D && (side || k == 0)) a.roots[4 * (side ? k + 1 : 0) + lane] = gl::from_mont(s);
+    }
+    if (in_range && lane == kW) {
+        u64 *bcol = a.out + (u64)kW * a.n + at;
+#pragma unroll
+        for (int r = 0; r < 8; r++) bcol[r] = bit ? gl::ONE : 0;
+    } else if (in_range && lane == kW + 1) {
+        u64 *icol = a.out + (u64)(kW + 1) * a.n + at;
+        const u64 v = gl::to_mont(idx >> a.j);
+#pragma unroll
+        for (int r = 0; r < 8; r++) icol[r] = v;
+    } else if (in_range && lane == kW + 2) {
+        u64 *scol = a.out + (u64)(kW + 2) * a.n + at;
+#pragma unroll
+        for (int r = 0; r < 8; r++) scol[r] = side ? gl::ONE : 0;
+    }
+}
+
+// the heap after the writes: node (2^D + i_k) >> j gets its last writer's new value, read from the new path (its input
+// at level j < D, its output at level D - 1 for the root, which only write K - 1 sets)
+__global__ void update_scatter_kernel(const u64 *indices, const unsigned char *last, const u64 *out, u64 K, u64 L,
+                                      u64 n, unsigned D, u64 *nodes) {
+    const u64 t = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (t >= (D + 1) * K) return;
+    const unsigned j = (unsigned)(t / K);
+    const u64 k = t % K;
+    if (j < D ? !last[t] : k != K - 1) return;
+    const u64 idx = indices[k], v = ((1ull << D) + idx) >> j;
+    const u64 row = j < D ? 8 * (L * (2 * k + 1) + j) : 8 * (L * (2 * k + 1) + D) - 1;
+    const unsigned half = j < D && ((idx >> j) & 1) ? 4 : 0;
+    for (int w = 0; w < 4; w++) nodes[4 * v + w] = gl::from_mont(out[(u64)(half + w) * n + row]);
+}
+
 static bool pow2(u64 v) { return v && !(v & (v - 1)); }
 static unsigned log2u(u64 v) { return 63 - __builtin_clzll(v); }
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 }  // namespace ms
 
@@ -370,4 +538,137 @@ extern "C" int ms_rescue_merkle_paths(ms_ctx *c, const void *nodes, uint32_t dep
     MS_CHECK_LAUNCH(c);
     const int rc_i = I.finish(), rc_n = N.finish(), rc_o = O.finish();
     return rc_i ? rc_i : rc_n ? rc_n : rc_o;
+}
+
+extern "C" int ms_rescue_merkle_updates(ms_ctx *c, void *nodes, uint32_t depth, const uint64_t *indices,
+                                        const uint64_t *new_leaves, uint64_t K, void *out, uint64_t *roots) {
+    if (!c) return MS_ERR_INVALID;
+    if (!nodes || !indices || !new_leaves || !out || !roots)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: null argument");
+    if (!pow2(K)) return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: K = %llu is not a power of two", (unsigned long long)K);
+    if (depth < 1 || depth > 32)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: depth %u is outside 1..32", (unsigned)depth);
+    const unsigned log_l = depth == 1 ? 0 : log2u(depth - 1) + 1;     // L = 2^log_l, the smallest power of two >= D
+    if (log2u(K) + log_l + 4 > 32)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: 16 K L rows (K = %llu, depth %u) exceed 2^32",
+                    (unsigned long long)K, (unsigned)depth);
+    const u64 L = 1ull << log_l, n = 16 * K * L;
+    const size_t kw = (size_t)K * 4 * 8;                               // one K x 4 word buffer
+    // scratch arena 3: the check flags, the sort's keys and values (double-buffered), the marks and their scan, the
+    // siblings, the old and new paths' inputs (double-buffered), the last-writer flags of levels 0..D-1, cub's storage
+    size_t sort_b = 0, scan_b = 0;
+    MS_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const u32 *)nullptr, (u32 *)nullptr, (const u32 *)nullptr,
+                                               (u32 *)nullptr, (int)K, 0, 32, c->stream));
+    MS_CUDA(c, cub::DeviceScan::InclusiveScan(nullptr, scan_b, (const UpdateMarks *)nullptr, (UpdateMarks *)nullptr,
+                                              UpdateMarksMax(), (int)K, c->stream));
+    const size_t u32s = align256((size_t)K * 4), marks_b = align256((size_t)K * sizeof(UpdateMarks));
+    const size_t off_keys = 256, off_marks = off_keys + 4 * u32s, off_sib = off_marks + 2 * marks_b,
+                 off_cur = off_sib + align256(kw), off_last = off_cur + 4 * align256(kw),
+                 off_temp = off_last + align256((size_t)K * depth), total = off_temp + (sort_b > scan_b ? sort_b : scan_b);
+    void *scr = nullptr;
+    if (int rc = scratch_get(c, 3, total, &scr)) return rc;
+    char *sb = (char *)scr;
+    unsigned long long *flag = (unsigned long long *)sb;
+    u32 *keys[2] = {(u32 *)(sb + off_keys), (u32 *)(sb + off_keys + u32s)};
+    u32 *vals[2] = {(u32 *)(sb + off_keys + 2 * u32s), (u32 *)(sb + off_keys + 3 * u32s)};
+    UpdateMarks *marks = (UpdateMarks *)(sb + off_marks), *scan = (UpdateMarks *)(sb + off_marks + marks_b);
+    u64 *sib = (u64 *)(sb + off_sib);
+    u64 *cur_old[2] = {(u64 *)(sb + off_cur), (u64 *)(sb + off_cur + align256(kw))};
+    u64 *cur_new[2] = {(u64 *)(sb + off_cur + 2 * align256(kw)), (u64 *)(sb + off_cur + 3 * align256(kw))};
+    unsigned char *last = (unsigned char *)(sb + off_last);
+    void *temp = sb + off_temp;
+
+    Staged I(c, indices, (size_t)K * 8, true, false);
+    if (I.rc) return I.rc;
+    Staged V(c, new_leaves, kw, true, false);
+    if (V.rc) return V.rc;
+    const u64 *idx = I.as<u64>();
+    MS_CUDA(c, cudaMemsetAsync(flag, 0xFF, 16, c->stream));
+    const u64 check_blocks = (4 * K + 255) / 256 < 1024 ? (4 * K + 255) / 256 : 1024;
+    update_check_kernel<<<(unsigned)check_blocks, 256, 0, c->stream>>>(idx, V.as<u64>(), K, 1ull << depth, cur_new[0], flag);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    u64 bad[2] = {0, 0}, value = 0;
+    MS_CUDA(c, cudaMemcpyAsync(bad, flag, 16, cudaMemcpyDeviceToHost, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (bad[0] != ~0ull) {
+        MS_CUDA(c, cudaMemcpy(&value, idx + bad[0], 8, cudaMemcpyDefault));
+        return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: index %llu of write %llu is not below 2^%u",
+                    (unsigned long long)value, (unsigned long long)bad[0], (unsigned)depth);
+    }
+    if (bad[1] != ~0ull) {
+        MS_CUDA(c, cudaMemcpy(&value, V.as<u64>() + bad[1], 8, cudaMemcpyDefault));
+        return fail(c, MS_ERR_INVALID, "ms_rescue_merkle_updates: word %llu of new leaf %llu (%llu) is not canonical",
+                    (unsigned long long)(bad[1] % 4), (unsigned long long)(bad[1] / 4), (unsigned long long)value);
+    }
+
+    Staged N(c, nodes, (size_t)(2ull << depth) * 4 * 8, true, true);
+    if (N.rc) return N.rc;
+    Staged O(c, out, (size_t)(kW + 3) * n * 8, false, true);
+    if (O.rc) return O.rc;
+    Staged R(c, roots, (size_t)(K + 1) * 4 * 8, false, true);
+    if (R.rc) return R.rc;
+    u64 *heap = N.as<u64>();
+    MS_CUDA(c, cudaMemsetAsync(last, 1, (size_t)K * depth, c->stream));
+    const unsigned kblocks = (unsigned)((K + kUpdateThreads - 1) / kUpdateThreads);
+    const unsigned pblocks = (unsigned)((2 * K * kLanes + kThreads - 1) / kThreads);
+    UpdateArgs u;
+    u.indices = idx;
+    u.roots = R.as<u64>();
+    u.K = K;
+    u.L = L;
+    u.n = n;
+    u.D = depth;
+    u.out = O.as<u64>();
+    int in = 0;                                                        // cur_*[in] holds this level's inputs
+    for (unsigned j = 0; j < L; j++) {
+        if (j < depth) {
+            const int bits = (int)depth - 1 - (int)j;                   // the parent's index below the top level
+            update_keys_kernel<<<kblocks, kUpdateThreads, 0, c->stream>>>(idx, K, j + 1, keys[0], vals[0]);
+            c->launches++;
+            MS_CHECK_LAUNCH(c);
+            const u32 *skeys = keys[0], *order = vals[0];
+            if (bits > 0) {
+                MS_CUDA(c, cub::DeviceRadixSort::SortPairs(temp, sort_b, keys[0], keys[1], vals[0], vals[1], (int)K, 0,
+                                                           bits, c->stream));
+                skeys = keys[1];
+                order = vals[1];
+            }
+            update_marks_kernel<<<kblocks, kUpdateThreads, 0, c->stream>>>(skeys, order, idx, K, j, marks);
+            c->launches++;
+            MS_CHECK_LAUNCH(c);
+            MS_CUDA(c, cub::DeviceScan::InclusiveScan(temp, scan_b, marks, scan, UpdateMarksMax(), (int)K, c->stream));
+            ResolveArgs r;
+            r.nodes = heap;
+            r.indices = idx;
+            r.order = order;
+            r.scan = scan;
+            r.cur_new = cur_new[in];
+            r.sib = sib;
+            r.cur_old = cur_old[in];
+            r.last = last + (size_t)j * K;
+            r.K = K;
+            r.D = depth;
+            r.j = j;
+            update_resolve_kernel<<<kblocks, kUpdateThreads, 0, c->stream>>>(r);
+            c->launches++;
+            MS_CHECK_LAUNCH(c);
+        }
+        u.cur_in[0] = cur_old[in];
+        u.cur_in[1] = cur_new[in];
+        u.cur_out[0] = cur_old[in ^ 1];
+        u.cur_out[1] = cur_new[in ^ 1];
+        u.sib = j < depth ? sib : nullptr;
+        u.j = j;
+        rescue_merkle_update_kernel<<<pblocks, kThreads, 0, c->stream>>>(u);
+        c->launches++;
+        MS_CHECK_LAUNCH(c);
+        in ^= 1;
+    }
+    const u64 sblocks = ((u64)(depth + 1) * K + kUpdateThreads - 1) / kUpdateThreads;
+    update_scatter_kernel<<<(unsigned)sblocks, kUpdateThreads, 0, c->stream>>>(idx, last, O.as<u64>(), K, L, n, depth, heap);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    const int rc_i = I.finish(), rc_v = V.finish(), rc_n = N.finish(), rc_o = O.finish(), rc_r = R.finish();
+    return rc_i ? rc_i : rc_v ? rc_v : rc_n ? rc_n : rc_o ? rc_o : rc_r;
 }
