@@ -454,6 +454,14 @@ class Context:
         self._ck(self.lib.ms_rescue_merkle_updates(self.h, _ptr(nodes), int(depth), _ptr(indices), _ptr(new_leaves),
                                                    int(K), _ptr(out), _ptr(roots)))
 
+    def rescue_rollup(self, nodes, depth, transfers, K, out, roots):
+        """apply K transfers in order to the accounts of the heap `nodes` of depth D, in place: transfers is (K, 3)
+        uint64 words (sender, receiver, amount); write `out`, the (23, 32 K L) trace, and `roots`, the (K + 1, 4) roots
+        before the first transfer and after each (all host or device; ms_rescue_rollup); synchronises.  An invalid
+        batch raises MsError naming its first failing transfer and writes nothing"""
+        self._ck(self.lib.ms_rescue_rollup(self.h, _ptr(nodes), int(depth), _ptr(transfers), int(K), _ptr(out),
+                                           _ptr(roots)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

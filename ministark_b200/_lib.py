@@ -22,6 +22,7 @@ RESCUE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_
 RESCUE_HASH_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_hash.h")
 RESCUE_MERKLE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle.h")
 RESCUE_MERKLE_UPDATES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle_updates.h")
+RESCUE_ROLLUP_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_rollup.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -144,6 +145,11 @@ _RESCUE_MERKLE_UPDATES_SIGS = {
     "ms_rescue_merkle_updates": (ci, [vp, vp, ui, vp, vp, u64, vp, vp]),
 }
 
+# include/ministark_rescue_rollup.h: the trace of examples/rollup's K balance transfers, and the heap after them
+_RESCUE_ROLLUP_SIGS = {
+    "ms_rescue_rollup": (ci, [vp, vp, ui, vp, u64, vp, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -183,6 +189,7 @@ def load():
         bind(lib, _RESCUE_HASH_SIGS)
         bind(lib, _RESCUE_MERKLE_SIGS)
         bind(lib, _RESCUE_MERKLE_UPDATES_SIGS)
+        bind(lib, _RESCUE_ROLLUP_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

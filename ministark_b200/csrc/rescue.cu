@@ -1,7 +1,8 @@
 // rescue.cu — the traces of examples/rescue and examples/merkle, side by side on the device: K independent chains of L
 // Rescue-Prime permutations (include/ministark_rescue.h), K messages absorbed by the Rescue-Prime sponge
 // (include/ministark_rescue_hash.h), the Rescue-Prime Merkle tree with K authentication paths through it
-// (include/ministark_rescue_merkle.h), and K ordered leaf writes into that tree (include/ministark_rescue_merkle_updates.h).
+// (include/ministark_rescue_merkle.h), K ordered leaf writes into that tree (include/ministark_rescue_merkle_updates.h),
+// and K balance transfers between the accounts that are its leaves (include/ministark_rescue_rollup.h).
 //
 // One chain (or message, tree node, path) per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's
 // parameters and write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the
@@ -14,6 +15,7 @@
 #include "../../include/ministark_rescue_hash.h"
 #include "../../include/ministark_rescue_merkle.h"
 #include "../../include/ministark_rescue_merkle_updates.h"
+#include "../../include/ministark_rescue_rollup.h"
 #include "ctx.cuh"
 #include "rescue_params.cuh"
 
@@ -398,6 +400,80 @@ __global__ void update_scatter_kernel(const u64 *indices, const unsigned char *l
     for (int w = 0; w < 4; w++) nodes[4 * v + w] = gl::from_mont(out[(u64)(half + w) * n + row]);
 }
 
+// ------------------------------------------------------------------------------------ examples/rollup: transfers
+// Transfer k is write 2 k (the sender step: delta = -amount, nonce + 1) then write 2 k + 1 (the receiver step: delta =
+// +amount).  Sorting the 2 K writes stably by account puts each account's writes in one run, in write order; an
+// inclusive scan of (delta, nonce increment) within the run then gives what the account's balance and nonce have
+// gained after each of its writes.
+struct RollupStep {
+    u64 delta, ninc;
+};
+
+struct RollupStepAdd {
+    __device__ __forceinline__ RollupStep operator()(const RollupStep &a, const RollupStep &b) const {
+        return {gl::add(a.delta, b.delta), gl::add(a.ninc, b.ninc)};
+    }
+};
+
+// the accounts below 2^D (the first failing 3 k + side) and the amounts below 2^32 (the first failing k), atomically;
+// per write w: its account as the updates' index and as the sort key, w as the sort value, and its delta
+__global__ void rollup_check_kernel(const u64 *transfers, u64 K, u64 bound, u64 *account, u32 *keys, u32 *vals,
+                                    u64 *delta, unsigned long long *first_bad) {
+    const u64 w = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (w >= 2 * K) return;
+    const u64 k = w >> 1, side = w & 1;
+    const u64 acc = transfers[3 * k + side], amount = transfers[3 * k + 2];
+    if (acc >= bound) atomicMin(first_bad, (unsigned long long)(3 * k + side));
+    if (side == 0 && amount >> 32) atomicMin(first_bad + 1, (unsigned long long)k);
+    const u64 a = acc < bound ? acc : 0, m = amount >> 32 ? 0 : amount;
+    account[w] = a;
+    keys[w] = (u32)a;
+    vals[w] = (u32)w;
+    delta[w] = side ? m : gl::sub(0, m);
+}
+
+__global__ void rollup_gather_kernel(const u32 *order, const u64 *delta, u64 n2, RollupStep *steps) {
+    const u64 t = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (t >= n2) return;
+    const u32 w = order[t];
+    steps[t] = {delta[w], (w & 1) ? 0ull : 1ull};
+}
+
+// write w's new leaf (balance + scanned delta, nonce + scanned increment, the owner words kept) and its new balance;
+// the lowest write whose new balance is not below 2^32, atomically
+__global__ void rollup_resolve_kernel(const u64 *nodes, const u32 *skeys, const u32 *order, const RollupStep *scan,
+                                      u64 n2, unsigned D, u64 *leaves, u64 *balance, unsigned long long *first_bad) {
+    const u64 t = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (t >= n2) return;
+    const u32 w = order[t];
+    const u64 *old = nodes + 4 * ((1ull << D) + skeys[t]);
+    const u64 bal = gl::add(old[0], scan[t].delta);
+    leaves[4 * (u64)w] = bal;
+    leaves[4 * (u64)w + 1] = gl::add(old[1], scan[t].ninc);
+    leaves[4 * (u64)w + 2] = old[2];
+    leaves[4 * (u64)w + 3] = old[3];
+    balance[w] = bal;
+    if (bal >> 32) atomicMin(first_bad, (unsigned long long)w);
+}
+
+// columns 15..22 of row i: on row 16 L w, write w's DELTA, NINC and balance limbs; M = 0; TBL = min(i, 255)
+__global__ void rollup_fill_kernel(const u64 *delta, const u64 *balance, u64 n, unsigned log_16l, u64 *out) {
+    const u64 i = blockIdx.x * (u64)kUpdateThreads + threadIdx.x;
+    if (i >= n) return;
+    u64 *col = out + (u64)(kW + 3) * n + i;
+    u64 v[6] = {0, 0, 0, 0, 0, 0};
+    if ((i & ((1ull << log_16l) - 1)) == 0) {
+        const u64 w = i >> log_16l, b = balance[w];
+        v[0] = gl::to_mont(delta[w]);
+        v[1] = (w & 1) ? 0 : gl::ONE;
+        for (int q = 0; q < 4; q++) v[2 + q] = gl::to_mont((b >> (8 * q)) & 255);
+    }
+#pragma unroll
+    for (int c = 0; c < 6; c++) col[(u64)c * n] = v[c];
+    col[6 * n] = 0;
+    col[7 * n] = gl::to_mont(i < 255 ? i : 255);
+}
+
 static bool pow2(u64 v) { return v && !(v & (v - 1)); }
 static unsigned log2u(u64 v) { return 63 - __builtin_clzll(v); }
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -671,4 +747,107 @@ extern "C" int ms_rescue_merkle_updates(ms_ctx *c, void *nodes, uint32_t depth, 
     MS_CHECK_LAUNCH(c);
     const int rc_i = I.finish(), rc_v = V.finish(), rc_n = N.finish(), rc_o = O.finish(), rc_r = R.finish();
     return rc_i ? rc_i : rc_v ? rc_v : rc_n ? rc_n : rc_o ? rc_o : rc_r;
+}
+
+extern "C" int ms_rescue_rollup(ms_ctx *c, void *nodes, uint32_t depth, const uint64_t *transfers, uint64_t K,
+                                void *out, uint64_t *roots) {
+    if (!c) return MS_ERR_INVALID;
+    if (!nodes || !transfers || !out || !roots) return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: null argument");
+    if (!pow2(K)) return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: K = %llu is not a power of two", (unsigned long long)K);
+    if (depth < 1 || depth > 32)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: depth %u is outside 1..32", (unsigned)depth);
+    const unsigned log_l = depth == 1 ? 0 : log2u(depth - 1) + 1;     // L = 2^log_l, the smallest power of two >= D
+    const unsigned log_n = log2u(K) + log_l + 5;
+    if (log_n > 32 || log_n < 8)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: 32 K L rows (K = %llu, depth %u) are not in 2^8..2^32",
+                    (unsigned long long)K, (unsigned)depth);
+    const u64 n = 1ull << log_n, n2 = 2 * K;
+    // scratch arena 2 (ms_rescue_merkle_updates takes arena 3): the check flags, the sort's keys and values
+    // (double-buffered), the accounts, the deltas, the steps and their scan, the new leaves and balances, the 2 K + 1
+    // roots of the writes, cub's storage
+    size_t sort_b = 0, scan_b = 0;
+    MS_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const u32 *)nullptr, (u32 *)nullptr, (const u32 *)nullptr,
+                                               (u32 *)nullptr, (int)n2, 0, (int)depth, c->stream));
+    MS_CUDA(c, cub::DeviceScan::InclusiveScanByKey(nullptr, scan_b, (const u32 *)nullptr, (const RollupStep *)nullptr,
+                                                   (RollupStep *)nullptr, RollupStepAdd(), (int)n2, cuda::std::equal_to<>(),
+                                                   c->stream));
+    const size_t u32s = align256(n2 * 4), words = align256(n2 * 8), steps_b = align256(n2 * sizeof(RollupStep));
+    const size_t off_keys = 256, off_acc = off_keys + 4 * u32s, off_delta = off_acc + words,
+                 off_steps = off_delta + words, off_leaves = off_steps + 2 * steps_b, off_bal = off_leaves + 4 * words,
+                 off_roots = off_bal + words, off_temp = off_roots + align256((n2 + 1) * 32),
+                 total = off_temp + (sort_b > scan_b ? sort_b : scan_b);
+    void *scr = nullptr;
+    if (int rc = scratch_get(c, 2, total, &scr)) return rc;
+    char *sb = (char *)scr;
+    unsigned long long *flag = (unsigned long long *)sb;
+    u32 *keys[2] = {(u32 *)(sb + off_keys), (u32 *)(sb + off_keys + u32s)};
+    u32 *vals[2] = {(u32 *)(sb + off_keys + 2 * u32s), (u32 *)(sb + off_keys + 3 * u32s)};
+    u64 *account = (u64 *)(sb + off_acc), *delta = (u64 *)(sb + off_delta);
+    RollupStep *steps = (RollupStep *)(sb + off_steps), *scan = (RollupStep *)(sb + off_steps + steps_b);
+    u64 *leaves = (u64 *)(sb + off_leaves), *balance = (u64 *)(sb + off_bal), *wroots = (u64 *)(sb + off_roots);
+    void *temp = sb + off_temp;
+
+    Staged T(c, transfers, (size_t)K * 3 * 8, true, false);
+    if (T.rc) return T.rc;
+    const unsigned blocks = (unsigned)((n2 + kUpdateThreads - 1) / kUpdateThreads);
+    MS_CUDA(c, cudaMemsetAsync(flag, 0xFF, 24, c->stream));
+    rollup_check_kernel<<<blocks, kUpdateThreads, 0, c->stream>>>(T.as<u64>(), K, 1ull << depth, account, keys[0],
+                                                                    vals[0], delta, flag);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    u64 bad[3] = {0, 0, 0}, value = 0;
+    MS_CUDA(c, cudaMemcpyAsync(bad, flag, 16, cudaMemcpyDeviceToHost, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (bad[0] != ~0ull) {
+        MS_CUDA(c, cudaMemcpy(&value, T.as<u64>() + bad[0], 8, cudaMemcpyDefault));
+        return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: %s %llu of transfer %llu is not below 2^%u",
+                    bad[0] % 3 ? "receiver" : "sender", (unsigned long long)value, (unsigned long long)(bad[0] / 3),
+                    (unsigned)depth);
+    }
+    if (bad[1] != ~0ull) {
+        MS_CUDA(c, cudaMemcpy(&value, T.as<u64>() + 3 * bad[1] + 2, 8, cudaMemcpyDefault));
+        return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: amount %llu of transfer %llu is not below 2^32",
+                    (unsigned long long)value, (unsigned long long)bad[1]);
+    }
+
+    Staged N(c, nodes, (size_t)(2ull << depth) * 4 * 8, true, true);
+    if (N.rc) return N.rc;
+    const u64 *heap = N.as<u64>();
+    MS_CUDA(c, cub::DeviceRadixSort::SortPairs(temp, sort_b, keys[0], keys[1], vals[0], vals[1], (int)n2, 0, (int)depth,
+                                               c->stream));
+    rollup_gather_kernel<<<blocks, kUpdateThreads, 0, c->stream>>>(vals[1], delta, n2, steps);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    MS_CUDA(c, cub::DeviceScan::InclusiveScanByKey(temp, scan_b, keys[1], steps, scan, RollupStepAdd(), (int)n2,
+                                                   cuda::std::equal_to<>(), c->stream));
+    rollup_resolve_kernel<<<blocks, kUpdateThreads, 0, c->stream>>>(heap, keys[1], vals[1], scan, n2, depth, leaves,
+                                                                      balance, flag + 2);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    MS_CUDA(c, cudaMemcpyAsync(bad + 2, flag + 2, 8, cudaMemcpyDeviceToHost, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (bad[2] != ~0ull) {
+        u64 acc = 0;
+        MS_CUDA(c, cudaMemcpy(&acc, account + bad[2], 8, cudaMemcpyDeviceToHost));
+        MS_CUDA(c, cudaMemcpy(&value, balance + bad[2], 8, cudaMemcpyDeviceToHost));
+        return fail(c, MS_ERR_INVALID, "ms_rescue_rollup: the %s step of transfer %llu leaves account %llu with balance "
+                    "%llu, not below 2^32", bad[2] & 1 ? "receiver" : "sender", (unsigned long long)(bad[2] / 2),
+                    (unsigned long long)acc, (unsigned long long)value);
+    }
+
+    Staged O(c, out, (size_t)(kW + 11) * n * 8, false, true);
+    if (O.rc) return O.rc;
+    Staged R(c, roots, (size_t)(K + 1) * 4 * 8, false, true);
+    if (R.rc) return R.rc;
+    // columns 0..14 of the (23, n) matrix are a (15, n) matrix: the updates trace of the 2 K writes
+    if (int rc = ms_rescue_merkle_updates(c, N.as<u64>(), depth, (const uint64_t *)account,
+                                          (const uint64_t *)leaves, n2, O.as<u64>(), (uint64_t *)wroots))
+        return rc;
+    MS_CUDA(c, cudaMemcpy2DAsync(R.as<u64>(), 32, wroots, 64, 32, K + 1, cudaMemcpyDeviceToDevice, c->stream));
+    const u64 fblocks = (n + kUpdateThreads - 1) / kUpdateThreads;
+    rollup_fill_kernel<<<(unsigned)fblocks, kUpdateThreads, 0, c->stream>>>(delta, balance, n, log_l + 4, O.as<u64>());
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    const int rc_t = T.finish(), rc_n = N.finish(), rc_o = O.finish(), rc_r = R.finish();
+    return rc_t ? rc_t : rc_n ? rc_n : rc_o ? rc_o : rc_r;
 }
