@@ -247,6 +247,14 @@ def test_pow_grind_smallest_nonce(ctx, orc):
     for tag, bits in ((b"a", 0), (b"b", 8), (b"c", 16), (b"d", 20)):
         seed = hashlib.sha256(tag).digest()
         assert ctx.pow_grind(seed, bits) == orc.pow_grind(seed, bits)
+    # each launch searches 2^24 nonces from `base` (1, 2^24 + 1, 2^25 + 1, ...): answers in the first, second and third
+    # launch.  The nonces are the serial CPU oracle's, re-derived in tests/test_oracle_pins.py.
+    for tag, bits, nonce in ((b"g0", 24, 10056532), (b"g2", 24, 28919286), (b"g5", 24, 41922605), (b"g3", 24, 45695959),
+                             (b"g0", 0, 1)):
+        seed = hashlib.sha256(tag).digest()
+        assert ctx.pow_grind(seed, bits) == nonce, (tag, bits)
+        digest = hashlib.sha256(seed + nonce.to_bytes(8, "big")).digest()
+        assert 256 - int.from_bytes(digest, "big").bit_length() >= bits
 
 
 @pytest.mark.parametrize("log_ff", [1, 2, 3, 4])

@@ -1,7 +1,8 @@
 """GPU: the "streamed_host" residency, whose Merkle node heaps live in pinned host memory (include/ministark_host_nodes.h,
 ministark_b200/prover.py, include/ministark_prover.hpp, tools/bf_cli.cpp --host-memory).
 
-  * ms_merkle_commit_block_sha256_host gives the local heaps and, with the top heap, the root of ms_merkle_commit_sha256;
+  * ms_merkle_commit_block_sha256_host gives the local heaps and, with the top heap, the root of ms_merkle_commit_sha256,
+    whose heap is the CPU oracle's;
   * it refuses pageable host memory and device memory with an error code;
   * the Python and C++ provers forced into streamed_host give the resident path's bytes on brainfuck at 2^16 and 2^20 rows,
     and the command line the recorded 2^20 proof;
@@ -36,17 +37,25 @@ def _matrix(ncols, N, field, seed):
     return torch.from_numpy(words.view(np.int64)).cuda()
 
 
-@pytest.mark.parametrize("field", [FP, FQ3])
-@pytest.mark.parametrize("log_N,log_b", [(12, 0), (12, 4), (14, 1), (16, 4), (16, 3)])
-def test_block_host_heaps_equal_the_device_tree(field, log_N, log_b):
+# five columns at every (log_N, log_b); the one-block (Fp 1, 7; Fq3 1, 3), constant-padding (Fp 8; Fq3 8 = 24 words)
+# and multi-block (Fp 17) leaf shapes at 16 blocks of 256 rows.  The five-column cases keep the ids they had before the
+# column count was a parameter.
+_HOST_CASES = ([(field, 5, log_N, log_b) for log_N, log_b in [(12, 0), (12, 4), (14, 1), (16, 4), (16, 3)] for field in [FP, FQ3]]
+               + [(FP, ncols, 12, 4) for ncols in (1, 7, 8, 17)] + [(FQ3, ncols, 12, 4) for ncols in (1, 3, 8)])
+
+
+@pytest.mark.parametrize("field,ncols,log_N,log_b", _HOST_CASES,
+                         ids=[f"{N}-{b}-{f}" + ("" if c == 5 else f"-{c}cols") for f, c, N, b in _HOST_CASES])
+def test_block_host_heaps_equal_the_device_tree(orc, field, ncols, log_N, log_b):
     ctx = Context(0)
-    N, beta, ncols = 1 << log_N, 1 << log_b, 5
+    N, beta = 1 << log_N, 1 << log_b
     log_n = log_N - log_b
     n = 1 << log_n
     mat = _matrix(ncols, N, field, seed=log_N * 10 + log_b + field)
     leaves, nodes = torch.empty((N, 4), dtype=torch.int64, device="cuda"), torch.empty((N, 4), dtype=torch.int64, device="cuda")
     root = ctx.merkle_commit(mat, field, N, ncols, leaves=leaves, nodes=nodes)
     want = nodes.cpu().numpy().view(np.uint8)
+    assert np.array_equal(want, orc.merkle_nodes(orc.hash_rows(mat.cpu().numpy().view(np.uint64), field)))
     local = torch.full((beta, n, 32), 0xAB, dtype=torch.uint8).pin_memory()
     top = torch.zeros((2 * beta, 4), dtype=torch.int64, device="cuda")
     torch.cuda.synchronize()                # the context runs on its own stream

@@ -69,10 +69,18 @@ def test_fib_native_size_verifies_and_trace_on_device(prover, orc):
         SO.verify(bad, proof.to_bytes(), fib.SECURITY_LEVEL, air_factory(bad))
 
 
+EVERY_SMALL_SET = "every index set of 1, 2 or 3 leaves"
+
+
 @pytest.mark.parametrize("n,ids", [(8, [3]), (4, [0, 1, 2, 3]), (1 << 10, [378]), (64, [5, 4, 63, 17, 16, 5]), (2, [1]),
-                                   (1 << 16, list(range(0, 1 << 16, 2049)))])
+                                   (1 << 16, list(range(0, 1 << 16, 2049))),
+                                   pytest.param(16, EVERY_SMALL_SET, id="16-every-set-of-1-2-3"),       # 696 sets, one tree
+                                   (16, [11, 4, 15, 0, 7, 4, 2, 13, 9, 1, 14, 6, 0, 10, 3, 12, 8, 5, 15, 11]),
+                                   (1 << 20, [int(i) for i in np.random.default_rng(64).integers(0, 1 << 20, size=64)]),
+                                   (1 << 20, [0, (1 << 20) - 1, (1 << 19) - 1, 1 << 19])])
 def test_merkle_prove_resident_tree(orc, n, ids):
     # MerkleTreeImpl::prove (src/merkle.rs:149-207; tests :528-581) from the device-resident leaf / node arrays
+    import itertools
     torch = pytest.importorskip("torch")
     from oracle import stark_oracle as SO
     ctx = ms.Context(0)
@@ -82,12 +90,14 @@ def test_merkle_prove_resident_tree(orc, n, ids):
     if n == 2:
         nodes[0] = 0          # nodes[0] is the unused default digest (src/merkle.rs:441)
     d_leaves, d_nodes = torch.from_numpy(leaves).cuda(), torch.from_numpy(nodes).cuda()
-    path, init, sib, height = ctx.merkle_prove(d_leaves, d_nodes, n, ids)
-    want = SO._merkle_prove(leaves, nodes, ids)
-    assert (path, init, sib, height) == (want["nodes"], want["initial_leaves"], want["sibling_leaves"], want["height"])
-    SO.merkle_verify(nodes[1].tobytes(), dict(nodes=path, initial_leaves=init, sibling_leaves=sib, height=height), ids)
-    # host-resident arrays go through the same kernel (staged)
-    assert ctx.merkle_prove(leaves, nodes, n, ids)[0] == path
+    sets = [ids] if ids is not EVERY_SMALL_SET else [list(s) for k in (1, 2, 3) for s in itertools.combinations(range(n), k)]
+    for ids in sets:
+        path, init, sib, height = ctx.merkle_prove(d_leaves, d_nodes, n, ids)
+        want = SO._merkle_prove(leaves, nodes, ids)
+        assert (path, init, sib, height) == (want["nodes"], want["initial_leaves"], want["sibling_leaves"], want["height"]), ids
+        SO.merkle_verify(nodes[1].tobytes(), dict(nodes=path, initial_leaves=init, sibling_leaves=sib, height=height), ids)
+        # host-resident arrays go through the same kernel (staged)
+        assert ctx.merkle_prove(leaves, nodes, n, ids)[0] == path
     with pytest.raises(ms.MsError):
         ctx.merkle_prove(d_leaves, d_nodes, n, [n])      # LeafIndexOutOfBounds
 

@@ -1,7 +1,8 @@
 """GPU: the streamed residency of `GpuProver` and its two kernels against their resident counterparts.
 
   * ms_merkle_commit_block_sha256 over every coset block, then ms_merkle_nodes_sha256 over the block roots, gives the
-    node heap and root of ms_merkle_commit_sha256 over the whole matrix, bit for bit;
+    node heap and root of ms_merkle_commit_sha256 over the whole matrix, bit for bit, and both equal the CPU oracle's
+    up to 2^16 rows; a single row, which ms_merkle_commit_sha256 refuses, gives its leaf digest as the block root;
   * ms_lde_rows gives the rows ms_gather_rows reads from ms_lde_batch(..., bitrev_out = 1);
   * a proof made with the budget forced between the two estimates (streamed) has the bytes of the resident prover's;
   * for brainfuck the streamed torch peak stays within its own estimate and far below the resident peak."""
@@ -30,17 +31,34 @@ def _rand(ctx, ncols, words, seed):
     return t
 
 
-@pytest.mark.parametrize("field", [ms.FP, ms.FQ3])
-@pytest.mark.parametrize("log_n", [0, 1, 5, 12, 20])
-@pytest.mark.parametrize("log_b", [0, 1, 3, 4])
-def test_block_commit_equals_resident_commit(ctx, field, log_n, log_b):
-    if log_n + log_b == 0:
-        pytest.skip("a Merkle tree needs two leaves")
+# (field, ncols): three columns at every block size; the other counts, without the 2^20-row blocks, put the one-block
+# (Fp 1, 7; Fq3 1), constant-padding (Fp 8; Fq3 8 = 24 words) and multi-block (Fp 17) leaf shapes through the block
+# commit.  The three-column cases keep the ids they had before the column count was a parameter.
+_BLOCK_CASES = [(field, ncols, log_n, log_b)
+                for field, ncols in [(ms.FP, 3), (ms.FQ3, 3), (ms.FP, 1), (ms.FP, 7), (ms.FP, 8), (ms.FP, 17), (ms.FQ3, 1),
+                                     (ms.FQ3, 8)]
+                for log_n in ([0, 1, 5, 12, 20] if ncols == 3 else [0, 1, 5, 12]) for log_b in [0, 1, 3, 4]]
+
+
+@pytest.mark.parametrize("field,ncols,log_n,log_b", _BLOCK_CASES,
+                         ids=[f"{b}-{n}-{f}" + ("" if c == 3 else f"-{c}cols") for f, c, n, b in _BLOCK_CASES])
+def test_block_commit_equals_resident_commit(ctx, orc, field, ncols, log_n, log_b):
     n, beta = 1 << log_n, 1 << log_b
-    N, ncols = n * beta, 3
+    N = n * beta
     mat = _rand(ctx, ncols, N * field, seed=log_n * 16 + log_b + field)
+    ctx.sync()
+    cols = np.ascontiguousarray(mat.cpu().numpy().view(np.uint64)) if N <= 1 << 16 else None
+    if N == 1:                                      # no tree: the resident commit refuses one leaf, the block root is it
+        with pytest.raises(ms.MsError):
+            ctx.merkle_commit(mat, field, N, ncols)
+        root = torch.empty(4, dtype=torch.int64, device="cuda")
+        ctx.merkle_commit_block(mat, field, 0, 0, 0, ncols, torch.empty(4, dtype=torch.int64, device="cuda"), root)
+        assert root.cpu().numpy().tobytes() == orc.hash_rows(cols, field)[0].tobytes()
+        return
     want = torch.empty((N, 4), dtype=torch.int64, device="cuda")
     root = ctx.merkle_commit(mat, field, N, ncols, nodes=want)
+    if cols is not None:                            # the resident commit itself against the serial CPU oracle
+        assert root == orc.merkle_nodes(orc.hash_rows(cols, field))[1].tobytes()
     nodes = torch.full((N, 4), -1, dtype=torch.int64, device="cuda")
     roots = torch.empty((beta, 4), dtype=torch.int64, device="cuda")
     for q in range(beta):

@@ -229,6 +229,13 @@ def test_pow_grind_vs_hashlib(orc):
         assert all(lz(k) < bits for k in range(1, nonce))
 
 
+def test_pow_grind_past_the_first_device_launch(orc):
+    # the serial search behind the 24-bit cases of tests/test_gpu_commit_stages_fri.py::test_pow_grind_smallest_nonce,
+    # whose answers lie in the first, second and third 2^24-nonce launch of the device grind (about 16 s on one core)
+    for tag, nonce in ((b"g0", 10056532), (b"g2", 28919286), (b"g5", 41922605), (b"g3", 45695959)):
+        assert orc.pow_grind(hashlib.sha256(tag).digest(), 24) == nonce, tag
+
+
 def test_scan_affine_oracle_vs_definition(orc):
     # x_0 = init, x_(i+1) = x_i * a_i + b_i in big-int Python
     n = 37
