@@ -462,6 +462,20 @@ class Context:
         self._ck(self.lib.ms_rescue_rollup(self.h, _ptr(nodes), int(depth), _ptr(transfers), int(K), _ptr(out),
                                            _ptr(roots)))
 
+    def rescue_wots_sign(self, secrets, seeds, messages, K, signatures, public_keys):
+        """sign messages[k] (K x 4 words) with the key of secrets[k] (K x 4) and seeds[k] (K x 2): write `signatures`
+        (K x 67 x 4 words) and `public_keys` (K x 6: the seed, then the root) (all host or device;
+        ms_rescue_wots_sign)"""
+        self._ck(self.lib.ms_rescue_wots_sign(self.h, _ptr(secrets), _ptr(seeds), _ptr(messages), int(K),
+                                              _ptr(signatures), _ptr(public_keys)))
+
+    def rescue_wots_trace(self, public_keys, messages, signatures, K, out):
+        """write `out`, the (15, 128 B) trace of K signatures (public_keys K x 6, messages K x 4, signatures K x 67 x 4
+        words; all host or device; ms_rescue_wots_trace); synchronises.  A signature that does not verify raises
+        MsError naming the lowest such k and writes nothing"""
+        self._ck(self.lib.ms_rescue_wots_trace(self.h, _ptr(public_keys), _ptr(messages), _ptr(signatures), int(K),
+                                               _ptr(out)))
+
 
 BF_SIZES = ("proc_rows", "instr_rows", "mem_rows", "reads", "writes", "n", "work_bytes")     # MS_BF_* of ministark_bf.h
 

@@ -23,6 +23,7 @@ RESCUE_HASH_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "minis
 RESCUE_MERKLE_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle.h")
 RESCUE_MERKLE_UPDATES_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_merkle_updates.h")
 RESCUE_ROLLUP_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_rollup.h")
+RESCUE_WOTS_HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ministark_rescue_wots.h")
 
 u64 = C.c_uint64
 vp = C.c_void_p
@@ -150,6 +151,12 @@ _RESCUE_ROLLUP_SIGS = {
     "ms_rescue_rollup": (ci, [vp, vp, ui, vp, u64, vp, vp]),
 }
 
+# include/ministark_rescue_wots.h: examples/wots's K one-time signatures, and the trace that proves them valid
+_RESCUE_WOTS_SIGS = {
+    "ms_rescue_wots_sign": (ci, [vp, vp, vp, vp, u64, vp, vp]),
+    "ms_rescue_wots_trace": (ci, [vp, vp, vp, vp, u64, vp]),
+}
+
 
 def bind(lib, sigs):
     for name, (res, args) in sigs.items():
@@ -190,6 +197,7 @@ def load():
         bind(lib, _RESCUE_MERKLE_SIGS)
         bind(lib, _RESCUE_MERKLE_UPDATES_SIGS)
         bind(lib, _RESCUE_ROLLUP_SIGS)
+        bind(lib, _RESCUE_WOTS_SIGS)
         if b"sm_90a" not in lib.ms_version():      # only the CUDA build is ever used: there is no CPU path in the product
             raise RuntimeError(f"{LIB_PATH} is not the sm_90a build of libministark_b200 ({lib.ms_version()!r})")
         _lib = lib

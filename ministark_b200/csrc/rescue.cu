@@ -2,7 +2,8 @@
 // Rescue-Prime permutations (include/ministark_rescue.h), K messages absorbed by the Rescue-Prime sponge
 // (include/ministark_rescue_hash.h), the Rescue-Prime Merkle tree with K authentication paths through it
 // (include/ministark_rescue_merkle.h), K ordered leaf writes into that tree (include/ministark_rescue_merkle_updates.h),
-// and K balance transfers between the accounts that are its leaves (include/ministark_rescue_rollup.h).
+// K balance transfers between the accounts that are its leaves (include/ministark_rescue_rollup.h), and K Winternitz
+// one-time signatures over the permutation (include/ministark_rescue_wots.h).
 //
 // One chain (or message, tree node, path) per 16 lanes (two per warp), one state word per lane; lanes 12-15 compute along on word 11's
 // parameters and write nothing.  A lane keeps its row of the MDS matrix and its 14 round constants in registers, so the
@@ -16,6 +17,7 @@
 #include "../../include/ministark_rescue_merkle.h"
 #include "../../include/ministark_rescue_merkle_updates.h"
 #include "../../include/ministark_rescue_rollup.h"
+#include "../../include/ministark_rescue_wots.h"
 #include "ctx.cuh"
 #include "rescue_params.cuh"
 
@@ -474,6 +476,157 @@ __global__ void rollup_fill_kernel(const u64 *delta, const u64 *balance, u64 n, 
     col[7 * n] = gl::to_mont(i < 255 ? i : 255);
 }
 
+// ------------------------------------------------------------------------- examples/wots: one-time signatures
+// One chain (signature element, trace block) per 16 lanes, as above.  Chain step s of chain i under seed rho permutes
+// (x || 0^4 || 1 + s, i, rho_0, rho_1), the chain secret (sigma || 0^4 || 16, i, rho), the fold (end || acc || 0, i, rho).
+constexpr unsigned kWotsChains = 67, kWotsSteps = 15, kWotsBlock = 128;
+
+// digit i of a four-word message: its nibbles for i < 64, then those of the checksum sum_(j<64) (15 - d_j)
+__device__ __forceinline__ unsigned wots_digit(const u64 *m, unsigned i) {
+    if (i < 64) return (unsigned)(m[i >> 4] >> (4 * (i & 15))) & 15;
+    unsigned c = 0;
+    for (unsigned j = 0; j < 64; j++) c += 15 - ((unsigned)(m[j >> 4] >> (4 * (j & 15))) & 15);
+    return (c >> (4 * (i - 64))) & 15;
+}
+
+// a permutation input on the group's lanes (all Montgomery): x on lanes 0..3, tail on 4..7, then the tweak, i, rho_0
+// and rho_1; lanes 12..15 take 0
+__device__ __forceinline__ u64 wots_input(unsigned lane, u64 x, u64 tail, u64 tweak, u64 i, u64 r0, u64 r1) {
+    return lane < 4 ? x : lane < 8 ? tail : lane == 8 ? tweak : lane == 9 ? i : lane == 10 ? r0 : lane == 11 ? r1 : 0;
+}
+
+// the permutation, its eight states written to col[0..7] when `live`
+__device__ __forceinline__ u64 wots_permute(const u64 (&row)[kW], const u64 (&c1)[kRounds], const u64 (&c2)[kRounds],
+                                            u64 s, u64 *col, bool live) {
+#pragma unroll
+    for (int r = 0; r < kRounds; r++) {
+        if (live) col[r] = s;
+        s = rescue_round(row, c1[r], c2[r], s);
+    }
+    if (live) col[kRounds] = s;
+    return s;
+}
+
+__global__ void wots_check_kernel(const u64 *v, u64 count, unsigned long long *first_bad) {
+    for (u64 t = blockIdx.x * (u64)blockDim.x + threadIdx.x; t < count; t += (u64)gridDim.x * blockDim.x)
+        if (v[t] >= gl::P) atomicMin(first_bad, (unsigned long long)t);
+}
+
+struct WotsSignArgs {
+    const u64 *secrets, *seeds, *messages;
+    u64 K;
+    u64 *signatures;            // K x 67 x 4 canonical
+    u64 *ends;                  // 67 K x 4 Montgomery
+};
+
+// chain c = 67 k + i: sk_i, then all 15 steps; the value before step d_i is signature element i
+__global__ void __launch_bounds__(kThreads) wots_sign_kernel(WotsSignArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 g = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool in_range = g < kWotsChains * a.K, out = in_range && lane < 4;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+    load_params(lane < (unsigned)kW ? lane : kW - 1, row, c1, c2);
+    const u64 c = in_range ? g : 0, k = c / kWotsChains;
+    const unsigned i = (unsigned)(c % kWotsChains), d = wots_digit(a.messages + 4 * k, i);
+    const u64 ti = gl::to_mont(i), r0 = gl::to_mont(a.seeds[2 * k]), r1 = gl::to_mont(a.seeds[2 * k + 1]);
+    u64 x = lane < 4 ? gl::to_mont(a.secrets[4 * k + lane]) : 0;
+    x = wots_permute(row, c1, c2, wots_input(lane, x, 0, gl::to_mont(16), ti, r0, r1), nullptr, false);
+    for (unsigned s = 0; s < kWotsSteps; s++) {
+        if (s == d && out) a.signatures[4 * c + lane] = gl::from_mont(x);
+        x = wots_permute(row, c1, c2, wots_input(lane, x, 0, gl::to_mont(1 + s), ti, r0, r1), nullptr, false);
+    }
+    if (d == kWotsSteps && out) a.signatures[4 * c + lane] = gl::from_mont(x);
+    if (out) a.ends[4 * c + lane] = x;
+}
+
+struct WotsFoldArgs {
+    const u64 *ends;            // 67 K x 4 Montgomery: the chain ends
+    const u64 *seeds;           // rho of key k at seeds[seed_stride k]
+    u64 seed_stride, K;
+    u64 *accs;                  // 67 K x 4 Montgomery: each fold's acc input (or nullptr)
+    u64 *public_keys;           // K x 6: (rho_0, rho_1, root) per key (or nullptr)
+    const u64 *expect;          // K x 6: the root each key must reach (or nullptr)
+    unsigned long long *first_bad;
+};
+
+// one key's 67 folds per 16 lanes, in order: acc <- words 0..3 of permute(end_i || acc || 0, i, rho), from acc = 0
+__global__ void __launch_bounds__(kThreads) wots_fold_kernel(WotsFoldArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 g0 = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool in_range = g0 < a.K, out = in_range && lane < 4;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+    load_params(lane < (unsigned)kW ? lane : kW - 1, row, c1, c2);
+    const u64 g = in_range ? g0 : 0;
+    const u64 r0 = gl::to_mont(a.seeds[a.seed_stride * g]), r1 = gl::to_mont(a.seeds[a.seed_stride * g + 1]);
+    u64 acc = 0;
+    for (unsigned i = 0; i < kWotsChains; i++) {
+        const u64 b = kWotsChains * g + i;
+        if (out && a.accs) a.accs[4 * b + lane] = acc;
+        const u64 x = lane < 4 ? a.ends[4 * b + lane] : 0;
+        const u64 tail = __shfl_sync(~0u, acc, lane & 3, kLanes);
+        acc = wots_permute(row, c1, c2, wots_input(lane, x, tail, 0, gl::to_mont(i), r0, r1), nullptr, false);
+    }
+    const u64 root = gl::from_mont(acc);
+    if (out && a.public_keys) {
+        a.public_keys[6 * g + 2 + lane] = root;
+        if (lane < 2) a.public_keys[6 * g + lane] = a.seeds[a.seed_stride * g + lane];
+    }
+    if (out && a.expect && a.expect[6 * g + 2 + lane] != root) atomicMin(a.first_bad, (unsigned long long)g);
+}
+
+struct WotsTraceArgs {
+    const u64 *public_keys, *messages, *signatures;
+    u64 K, B, n;
+    const u64 *accs;            // per block, Montgomery (kWrite)
+    u64 *ends;                  // per block, Montgomery (!kWrite)
+    u64 *out;
+};
+
+// block b per 16 lanes: the 15 chain slots from the signature element (0 for padding), each step applied from slot
+// d on.  kWrite = false: the chain end into ends.  kWrite = true: the block's rows, the fold on accs[b] included (on 0^4
+// for padding, which has LAST = 1 and so follows a block with LAST = 1); lane 12 writes ACT, lane 13 CNT, lane 14 LAST
+template <bool kWrite>
+__global__ void __launch_bounds__(kThreads) wots_trace_kernel(WotsTraceArgs a) {
+    const unsigned lane = threadIdx.x % kLanes;
+    const u64 g = (blockIdx.x * (u64)kThreads + threadIdx.x) / kLanes;
+    const bool in_range = g < a.B, live = kWrite && in_range && lane < (unsigned)kW;
+    const unsigned w = lane < (unsigned)kW ? lane : kW - 1;
+    u64 row[kW], c1[kRounds], c2[kRounds];
+    load_params(w, row, c1, c2);
+    const u64 b = in_range ? g : 0, k = b / kWotsChains;
+    const bool real = k < a.K;
+    const unsigned i = real ? (unsigned)(b % kWotsChains) : 0, d = real ? wots_digit(a.messages + 4 * k, i) : 0;
+    const u64 last = !real || i == kWotsChains - 1 ? gl::ONE : 0;
+    const u64 ti = gl::to_mont(i), r0 = real ? gl::to_mont(a.public_keys[6 * k]) : 0,
+              r1 = real ? gl::to_mont(a.public_keys[6 * k + 1]) : 0;
+    u64 x = real && lane < 4 ? gl::to_mont(a.signatures[4 * b + lane]) : 0;
+    u64 *col = kWrite ? a.out + (u64)w * a.n + kWotsBlock * b : nullptr;
+    u64 *aux = kWrite ? a.out + (u64)(lane < kW + 3 ? lane : kW) * a.n + kWotsBlock * b : nullptr;
+    const bool aux_live = kWrite && in_range && lane >= (unsigned)kW && lane < (unsigned)kW + 3;
+    for (unsigned s = 0; s < kWotsSteps; s++, col += 8, aux += 8) {
+        const u64 y = wots_permute(row, c1, c2, wots_input(lane, x, 0, gl::to_mont(1 + s), ti, r0, r1), col, live);
+        if (s >= d) x = y;
+        if (aux_live) {
+            const u64 v = lane == (unsigned)kW ? (s >= d ? gl::ONE : 0)
+                          : lane == (unsigned)kW + 1 ? gl::to_mont(s < d ? d - s : 0)
+                          : last;
+#pragma unroll
+            for (int r = 0; r < 8; r++) aux[r] = v;
+        }
+    }
+    if (!kWrite) {
+        if (in_range && lane < 4) a.ends[4 * b + lane] = x;
+        return;
+    }
+    const u64 tail = real && lane >= 4 && lane < 8 ? a.accs[4 * b + lane - 4] : 0;
+    wots_permute(row, c1, c2, wots_input(lane, x, tail, 0, ti, r0, r1), col, live);
+    if (aux_live) {
+        const u64 v = lane == (unsigned)kW + 2 ? last : 0;
+#pragma unroll
+        for (int r = 0; r < 8; r++) aux[r] = v;
+    }
+}
+
 static bool pow2(u64 v) { return v && !(v & (v - 1)); }
 static unsigned log2u(u64 v) { return 63 - __builtin_clzll(v); }
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -850,4 +1003,133 @@ extern "C" int ms_rescue_rollup(ms_ctx *c, void *nodes, uint32_t depth, const ui
     MS_CHECK_LAUNCH(c);
     const int rc_t = T.finish(), rc_n = N.finish(), rc_o = O.finish(), rc_r = R.finish();
     return rc_t ? rc_t : rc_n ? rc_n : rc_o ? rc_o : rc_r;
+}
+
+// the lowest index of each of `count` arrays whose word is not canonical, into flag[0..count), ~0 where none
+static int wots_check_words(ms_ctx *c, const u64 *const *arrays, const u64 *sizes, int count, unsigned long long *flag,
+                            u64 *bad) {
+    MS_CUDA(c, cudaMemsetAsync(flag, 0xFF, 8 * count, c->stream));
+    for (int q = 0; q < count; q++) {
+        const u64 blocks = (sizes[q] + 255) / 256 < 1024 ? (sizes[q] + 255) / 256 : 1024;
+        wots_check_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(arrays[q], sizes[q], flag + q);
+        c->launches++;
+        MS_CHECK_LAUNCH(c);
+    }
+    MS_CUDA(c, cudaMemcpyAsync(bad, flag, 8 * count, cudaMemcpyDeviceToHost, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    return MS_OK;
+}
+
+static int wots_fold(ms_ctx *c, const WotsFoldArgs &a) {
+    const u64 blocks = (a.K * kLanes + kThreads - 1) / kThreads;
+    wots_fold_kernel<<<(unsigned)blocks, kThreads, 0, c->stream>>>(a);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    return MS_OK;
+}
+
+extern "C" int ms_rescue_wots_sign(ms_ctx *c, const uint64_t *secrets, const uint64_t *seeds, const uint64_t *messages,
+                                   uint64_t K, void *signatures, void *public_keys) {
+    if (!c) return MS_ERR_INVALID;
+    if (!secrets || !seeds || !messages || !signatures || !public_keys)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_wots_sign: null argument");
+    if (K < 1 || K > MS_WOTS_MAX_KEYS)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_wots_sign: K = %llu is outside 1..%u", (unsigned long long)K,
+                    MS_WOTS_MAX_KEYS);
+    const u64 chains = kWotsChains * K;
+    // scratch arena 3: the check flags, then the chain ends
+    void *scr = nullptr;
+    if (int rc = scratch_get(c, 3, 256 + align256(chains * 32), &scr)) return rc;
+    unsigned long long *flag = (unsigned long long *)scr;
+    u64 *ends = (u64 *)((char *)scr + 256);
+    Staged S(c, secrets, (size_t)K * 32, true, false);
+    if (S.rc) return S.rc;
+    Staged D(c, seeds, (size_t)K * 16, true, false);
+    if (D.rc) return D.rc;
+    Staged M(c, messages, (size_t)K * 32, true, false);
+    if (M.rc) return M.rc;
+    const u64 *arrays[3] = {S.as<u64>(), D.as<u64>(), M.as<u64>()}, sizes[3] = {4 * K, 2 * K, 4 * K};
+    const char *names[3] = {"secret", "seed", "message"};
+    const unsigned widths[3] = {4, 2, 4};
+    u64 bad[3], value = 0;
+    if (int rc = wots_check_words(c, arrays, sizes, 3, flag, bad)) return rc;
+    for (int q = 0; q < 3; q++)
+        if (bad[q] != ~0ull) {
+            MS_CUDA(c, cudaMemcpy(&value, arrays[q] + bad[q], 8, cudaMemcpyDefault));
+            return fail(c, MS_ERR_INVALID, "ms_rescue_wots_sign: word %llu of %s %llu (%llu) is not canonical",
+                        (unsigned long long)(bad[q] % widths[q]), names[q], (unsigned long long)(bad[q] / widths[q]),
+                        (unsigned long long)value);
+        }
+    Staged G(c, signatures, (size_t)chains * 32, false, true);
+    if (G.rc) return G.rc;
+    Staged Pk(c, public_keys, (size_t)K * 48, false, true);
+    if (Pk.rc) return Pk.rc;
+    WotsSignArgs s{S.as<u64>(), D.as<u64>(), M.as<u64>(), K, G.as<u64>(), ends};
+    wots_sign_kernel<<<(unsigned)((chains * kLanes + kThreads - 1) / kThreads), kThreads, 0, c->stream>>>(s);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    if (int rc = wots_fold(c, {ends, D.as<u64>(), 2, K, nullptr, Pk.as<u64>(), nullptr, nullptr}))
+        return rc;
+    const int rc_s = S.finish(), rc_d = D.finish(), rc_m = M.finish(), rc_g = G.finish(), rc_p = Pk.finish();
+    return rc_s ? rc_s : rc_d ? rc_d : rc_m ? rc_m : rc_g ? rc_g : rc_p;
+}
+
+extern "C" int ms_rescue_wots_trace(ms_ctx *c, const uint64_t *public_keys, const uint64_t *messages,
+                                    const uint64_t *signatures, uint64_t K, void *out) {
+    if (!c) return MS_ERR_INVALID;
+    if (!public_keys || !messages || !signatures || !out)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_wots_trace: null argument");
+    if (K < 1 || K > MS_WOTS_MAX_KEYS)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_wots_trace: K = %llu is outside 1..%u", (unsigned long long)K,
+                    MS_WOTS_MAX_KEYS);
+    const u64 chains = kWotsChains * K, B = 1ull << (log2u(chains - 1) + 1), n = kWotsBlock * B;
+    // scratch arena 3: the check flags, the signatures' chain ends, their folds' acc inputs (padding blocks need
+    // neither: each is the same block, its fold on 0^4)
+    void *scr = nullptr;
+    if (int rc = scratch_get(c, 3, 256 + 2 * align256(chains * 32), &scr)) return rc;
+    unsigned long long *flag = (unsigned long long *)scr;
+    u64 *ends = (u64 *)((char *)scr + 256), *accs = (u64 *)((char *)scr + 256 + align256(chains * 32));
+    Staged Pk(c, public_keys, (size_t)K * 48, true, false);
+    if (Pk.rc) return Pk.rc;
+    Staged M(c, messages, (size_t)K * 32, true, false);
+    if (M.rc) return M.rc;
+    Staged S(c, signatures, (size_t)chains * 32, true, false);
+    if (S.rc) return S.rc;
+    const u64 *arrays[3] = {Pk.as<u64>(), M.as<u64>(), S.as<u64>()}, sizes[3] = {6 * K, 4 * K, 4 * chains};
+    const char *names[3] = {"public key", "message", "signature element"};
+    const unsigned widths[3] = {6, 4, 4};
+    u64 bad[3], value = 0;
+    if (int rc = wots_check_words(c, arrays, sizes, 3, flag, bad)) return rc;
+    for (int q = 0; q < 3; q++)
+        if (bad[q] != ~0ull) {
+            MS_CUDA(c, cudaMemcpy(&value, arrays[q] + bad[q], 8, cudaMemcpyDefault));
+            const u64 item = bad[q] / widths[q];
+            if (q == 2)
+                return fail(c, MS_ERR_INVALID, "ms_rescue_wots_trace: word %llu of element %llu of signature %llu (%llu) "
+                            "is not canonical", (unsigned long long)(bad[q] % 4), (unsigned long long)(item % kWotsChains),
+                            (unsigned long long)(item / kWotsChains), (unsigned long long)value);
+            return fail(c, MS_ERR_INVALID, "ms_rescue_wots_trace: word %llu of %s %llu (%llu) is not canonical",
+                        (unsigned long long)(bad[q] % widths[q]), names[q], (unsigned long long)item,
+                        (unsigned long long)value);
+        }
+    WotsTraceArgs t{Pk.as<u64>(), M.as<u64>(), S.as<u64>(), K, chains, n, accs, ends, nullptr};
+    wots_trace_kernel<false><<<(unsigned)((chains * kLanes + kThreads - 1) / kThreads), kThreads, 0, c->stream>>>(t);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    MS_CUDA(c, cudaMemsetAsync(flag, 0xFF, 8, c->stream));
+    if (int rc = wots_fold(c, {ends, Pk.as<u64>(), 6, K, accs, nullptr, Pk.as<u64>(), flag})) return rc;
+    MS_CUDA(c, cudaMemcpyAsync(bad, flag, 8, cudaMemcpyDeviceToHost, c->stream));
+    MS_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (bad[0] != ~0ull)
+        return fail(c, MS_ERR_INVALID, "ms_rescue_wots_trace: signature %llu does not verify: its root differs from its "
+                    "public key", (unsigned long long)bad[0]);
+    Staged O(c, out, (size_t)(kW + 3) * n * 8, false, true);
+    if (O.rc) return O.rc;
+    t.B = B;
+    t.out = O.as<u64>();
+    wots_trace_kernel<true><<<(unsigned)((B * kLanes + kThreads - 1) / kThreads), kThreads, 0, c->stream>>>(t);
+    c->launches++;
+    MS_CHECK_LAUNCH(c);
+    const int rc_p = Pk.finish(), rc_m = M.finish(), rc_s = S.finish(), rc_o = O.finish();
+    return rc_p ? rc_p : rc_m ? rc_m : rc_s ? rc_s : rc_o;
 }
